@@ -1,10 +1,10 @@
-# Build of the B200-native Pire scan path.
+# Build of the H100-native (sm_90a) Pire scan path.
 #   make            product library (pire_b200/libpire_b200.so) + oracle restatement
 #   make ref        the real reference compiled from /root/reference into oracle/_ref
 #   make microbench load-path / step-scheme microbenchmarks (tools/)
 NVCC      ?= nvcc
 CC        ?= gcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVCCFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -Wall -Xptxas -v
 
 CSRC      := pire_b200/csrc

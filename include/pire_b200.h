@@ -1,4 +1,4 @@
-/* pire_b200.h -- C ABI of the B200-native Pire scan path.
+/* pire_b200.h -- C ABI of the GPU-native (H100, sm_90a) Pire scan path.
  *
  * The reference (yandex/pire) has no plugin/FFI layer: its seam is the
  * compile-time "Scanner concept" consumed by the templates of pire/run.h

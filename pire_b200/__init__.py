@@ -1,7 +1,7 @@
-"""pire_b200 -- B200-native implementation of Pire's inner DFA scan path.
+"""pire_b200 -- H100-native (sm_90a) implementation of Pire's inner DFA scan path.
 
 Only what the path needs lives here:
-    csrc/         sm_100a CUDA kernels + the extern "C" boundary (include/pire_b200.h)
+    csrc/         sm_90a CUDA kernels + the extern "C" boundary (include/pire_b200.h)
     _native.py    ctypes binding of that boundary (fails loudly if the .so is missing)
     scanner.py    Python mirror of Pire's Scanner / Runner / Matches for batches
     workloads.py  the BASELINE.json pattern sets and synthetic corpora

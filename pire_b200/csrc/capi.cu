@@ -2,7 +2,7 @@
 //
 // Host side of the scan path: ingest the reference's Scanner::Save() stream
 // (pire_image.cpp), build and upload the device tables (dfa_tables.cpp), launch
-// the sm_100a kernels (scan_kernels.cu).  There is deliberately no CPU scan
+// the sm_90a kernels (scan_kernels.cu).  There is deliberately no CPU scan
 // here: without a CUDA device every run entry point fails with
 // PIRE_GPU_ENODEVICE.
 #include "capi_internal.hpp"
@@ -64,11 +64,10 @@ uint32_t ResolveVariant(const pire_gpu_scanner* sc, bool uniform)
     // AUTO: predication pays when lanes outside the resident state would
     // collide with it in the banks, i.e. for large (glued) automata -- in the uniform kernel, which is bound
     // by shared-memory wavefronts.  The CSR kernels (generic, lines) are bound by instruction issue on short
-    // strings, where the filter's two extra instructions per byte cost more than the conflicts they save
-    // (lines of text, glued ten: 903 GB/s plain, 717 pred).
+    // strings, where the filter's two extra instructions per byte cost more than the conflicts they save.
     if (!uniform)
         return PIRE_GPU_VARIANT_PLAIN;
-    // round 2: the look-ahead filter (5.5 instructions per byte, two strings per lane) beats the exit filter by 9 % on the
+    // the look-ahead filter (5.5 instructions per byte, two strings per lane) is chosen over the exit filter for the
     // glued benchmark scanner; it needs the look-ahead set (every exit of the resting state hot)
     if (sc->tab.states > 64)
         return sc->tab.look_ok ? PIRE_GPU_VARIANT_LOOK : PIRE_GPU_VARIANT_PRED;
@@ -379,7 +378,7 @@ static int PrefixOrSuffix(const pire_gpu_scanner* sc, const uint8_t* d_corpus, c
     a.uniform = (!reverse && IsUniform(d_corpus, d_offsets, fixed_len) && !getenv("PIRE_B200_NO_UNIFORM_BODY")) ? 1 : 0;
     if (a.uniform) {
         // the uniform prefix kernel walks plain: with the exit filter of hot id 0 its step is five ALU-pipe instructions
-        // (PRMT, SHF, 2 x LOP3, VIMNMX) and measured half the speed (1.64 vs 3.17 TB/s on the glued scanner);
+        // (PRMT, SHF, 2 x LOP3, VIMNMX), about twice the plain step's;
         // PIRE_B200_PREFIX_PRED=1 selects the filtered walk for experiments
         static const int forced = [] {
             const char* env = getenv("PIRE_B200_PREFIX_PRED");
@@ -903,6 +902,6 @@ int pire_gpu_synth_mixed_fill_host(uint64_t seed, uint32_t plant_every, uint64_t
 
 const char* pire_gpu_last_error(void) { return g_error.c_str(); }
 
-const char* pire_gpu_version(void) { return "pire-b200 0.1 (sm_100a)"; }
+const char* pire_gpu_version(void) { return "pire-b200 0.1 (sm_90a)"; }
 
 } // extern "C"

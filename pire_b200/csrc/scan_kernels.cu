@@ -1,4 +1,4 @@
-// scan_kernels.cu -- hand-written sm_100a kernels for Pire's inner scan loop.
+// scan_kernels.cu -- hand-written sm_90a kernels for Pire's inner scan loop.
 //
 // Replaces, for a batch of strings, the reference's
 //     Runner(sc).Begin().Run(ptr,len).End()   (pire/run.h:365-392)
@@ -22,9 +22,9 @@
 //   * LOOK variant (the glued benchmark scan): the filter looks one byte further -- a resting
 //     lane reads the table only if this byte and the next both pass -- in 5.5 instructions per
 //     byte (LookProbe / LookStep), two strings per lane (ScanUniformLook2Kernel).
-//   * Input bytes: each lane streams its own string: 32-byte read-only loads that
-//     bypass L1 allocation, one ahead in a register ping-pong (uniform kernels,
-//     LDG.256), or a four-deep cp.async ring of 16-byte chunks in shared memory
+//   * Input bytes: each lane streams its own string: 32-byte read-only loads (two
+//     LDG.128 of one sector, the second an L1 hit), one ahead in a register ping-pong (uniform kernels,
+//     two LDG.128 per 32 bytes), or a four-deep cp.async ring of 16-byte chunks in shared memory
 //     (CSR kernels).  Long strings of a length-ordered batch are split over a warp
 //     (ScanSplitKernel); lines of text are scanned in stream (ScanTextKernel).
 //   * Prefix / suffix scans and HalfFinalScanner counting reuse the walk; final hot
@@ -66,6 +66,15 @@ constexpr int kMinBlocksPerSM = 3;
 // dependent LDS chain per string), which fewer co-resident warps shorten.
 constexpr int kGenericBlocksPerSM = 2;
 constexpr int kWarpsPerBlock = kBlock / 32;
+// Grid cap of the grid-stride helper kernels (line counting, synthesis, accept gathering): `per_sm` CTAs on every SM
+// of the current device.
+unsigned long long GridCap(unsigned per_sm)
+{
+    int device = 0, sms = 0;
+    if (cudaGetDevice(&device) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms < 1)
+        sms = 1;
+    return (unsigned long long) sms * per_sm;
+}
 
 std::atomic<uint64_t> g_launches{0};
 
@@ -140,17 +149,22 @@ __device__ __forceinline__ void PrefetchL2(const uint8_t* p)
 }
 
 // The same load with a 256-byte L2 prefetch: the first touch of a 256-byte region of a string brings all of it
-// into L2, so the following seven 32-byte loads of the lane are L2 hits.
+// into L2, so the following seven 32-byte loads of the lane are L2 hits.  sm_90 has no 256-bit load: the 32 bytes
+// are two 128-bit loads of the same sector, issued back to back.  Both allocate in L1, so the second half of the
+// sector is an L1 hit; with L1::no_allocate both halves went to L2, and on an H100 the scans ran at about 0.55 of
+// the speed (glued scan 769 against 1393 GB/s, same build otherwise).
 __device__ __forceinline__ void LoadStream32P(const uint8_t* p, uint4& a, uint4& b)
 {
-    asm volatile("ld.global.nc.L1::no_allocate.L2::256B.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.L2::256B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
                  : "l"(p));
 }
 
 __device__ __forceinline__ void LoadStream32(const uint8_t* p, uint4& a, uint4& b)
 {
-    asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                 "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
                  : "l"(p));
 }
@@ -262,9 +276,8 @@ __device__ __forceinline__ void FastStep(const Tables& t, uint32_t& g, uint32_t 
     // Entry of (id g, byte b) sits at base + g * kHotStride + b.  `bb` = base | b comes from one PRMT (the
     // base is 256-byte aligned, so its low byte is free) and does not depend on g: the dependent chain of a
     // step is IMAD (FMA pipe) -> LDS, as short as the PRMT -> LDS of an unpadded table.
-    // byte `sel` + base: IDP.4A on the FMA pipe (round 2: +0.6 % on the exit-filter scan, +1-2 % on the CSR and counting
-    // kernels, which are short of ALU slots), or PRMT on the ALU pipe for the prefix kernels, whose look-ahead pass keeps
-    // the FMA side busy (IDP there measured 17 % slower)
+    // byte `sel` + base: IDP.4A on the FMA pipe (the scan, CSR and counting kernels are short of ALU slots), or PRMT on
+    // the ALU pipe for the prefix kernels, whose look-ahead pass keeps the FMA side busy
     const uint32_t bb = kIdp ? __dp4a(w, 1u << (8 * (sel & 3u)), t.base) : __byte_perm(w, t.base, 0x7650u | (sel & 3u));
     if (kPred) {
         // bit (byte & 31) of the 32-slot exit bitmap: may this byte leave hot id 0?
@@ -415,7 +428,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanUniformKernel(con
 
         if (len != 0) {
             // Two register sets in ping-pong: the 32 bytes after the ones being walked are
-            // always in flight (software prefetch, one LDG.256 per lane per 32 bytes).
+            // always in flight (software prefetch, one pair of LDG.128 per lane per 32 bytes).
             uint4 a0, a1, b0, b1;
             LoadStream32(p, a0, a1);
             for (uint32_t off = 0;;) {
@@ -477,7 +490,7 @@ struct LookFilter {
 // kClean: the probe's bit is moved to bit 31 with the bits below it cleared by one multiply (IMAD, FMA pipe: pa * 2^31
 // keeps bit 0 only), so that "both bytes pass, or the lane is outside id 0" is ONE LOP3 with a predicate result over
 // (pa, pa_next, g) instead of two: the step keeps six instructions, but two instead of three of them are on the
-// half-rate ALU pipe that ncu shows 66 % busy under the look-ahead kernel.
+// half-rate ALU pipe, which the look-ahead kernel keeps busy.
 template <bool k64, int kByte, bool kClean = false>
 __device__ __forceinline__ void LookProbe(uint32_t w, uint32_t base, const LookFilter& f, uint32_t& bb, uint32_t& pa)
 {
@@ -534,7 +547,7 @@ __device__ __forceinline__ void LookStep(uint32_t& g, uint32_t bb, uint32_t pa, 
 
 // Four bytes.  (bb0, pa0) belong to byte 0 of `w` and were computed by the previous call; pan is the probe of the
 // byte that follows the word.  (Looking ahead from the even bytes only -- half a LOP3 less per byte, 1.91 instead of
-// 1.72 wavefronts per step in the model -- measured slower, 2.67 vs 2.63 ms: profiles/r02_experiments_notes.txt.)
+// 1.72 wavefronts per step in the host model, tools/model_look.cpp -- is not done: it was slower when tried.)
 template <bool k64, bool kClean = false>
 __device__ __forceinline__ void LookWord(uint32_t& g, uint32_t w, uint32_t bb0, uint32_t pa0, uint32_t pan, uint32_t base,
                                          const LookFilter& f)
@@ -558,7 +571,7 @@ __device__ __forceinline__ uint32_t SmemWindowBase()
     return v;
 }
 
-// Thirty-two bytes (one LDG.256 per lane).  next0 = the word that follows the block (ignored when !more: the last
+// Thirty-two bytes (one pair of LDG.128 per lane).  next0 = the word that follows the block (ignored when !more: the last
 // byte of a string is filtered alone).  A lane that left the hot rows reads the sink row from then on; one test
 // per block finds it and replays both 16-byte chunks through the complete table.
 // Lane state in two registers: g (hot id, H = outside the hot rows) and prev = the complete state the lane had when
@@ -596,7 +609,7 @@ __device__ __forceinline__ void LookBlock32(const Tables& t, uint32_t& g, uint32
     LookWord<k64, kClean>(g, v1.z, bb, pa, pn, t.base, f);
     // The word after the block was requested from HBM when this block began: its probe must stay down here (an
     // ordinary intrinsic is hoisted to the top of the block by the compiler, where it waits for the whole DRAM
-    // latency -- ncu: 10 % of all stall samples on that one IDP).
+    // latency).
     // (a volatile mov is not enough: ptxas schedules across it.  The word is made to depend on the walk itself --
     // plus g times a kernel argument that is always zero -- which costs one IMAD per block.)
     const uint32_t late = next0 + g * opaque_zero;
@@ -611,7 +624,7 @@ __device__ __forceinline__ void LookBlock32(const Tables& t, uint32_t& g, uint32
 // Register budget.  The register file is split between the four warp schedulers (16 K registers each), so a
 // CTA's warps should be a multiple of four: 512 threads x 3 CTAs leaves 40 registers per thread (12 warps x 1280
 // per scheduler), 384 threads x 3 CTAs or 640 threads x 2 CTAs leave 48 (9 / 10 warps x 1536).  The kernel is short
-// of independent chains, so the ten-warp shape wins (2.423 ms against 2.480 on the glued scan); both instantiations
+// of independent chains, so the ten-warp shape is the default; both instantiations
 // exist (PIRE_B200_LOOK_REGS=40|48, PIRE_B200_LOOK_BLOCK=<threads> for experiments).
 constexpr int kLookBlock40 = 512;
 constexpr int kLookBlock48 = 640;
@@ -668,10 +681,9 @@ __global__ void __maxnreg__(kRegs) ScanUniformLookKernel(const __grid_constant__
                     p += 32;
                     if (more_a)
                         LoadStream32(p, a0, a1);
-                    // The warp barrier pins the load HERE.  Left alone, the scheduler sinks the LDG.256 towards its first
-                    // use to lend its eight destination registers to the steps in between (SASS: issued 7 steps before
-                    // the block's end instead of 32), which exposes most of a DRAM round trip per block (ncu: 14 % of all
-                    // stall samples were long-scoreboard waits on the first use of the loaded word).
+                    // The warp barrier pins the loads HERE.  Left alone, the scheduler sinks the two LDG.128 towards
+                    // their first use to lend their eight destination registers to the steps in between, which exposes
+                    // most of a DRAM round trip per block (long-scoreboard waits on the first use of the loaded word).
                     __syncwarp();
                     LookBlock32<k64, kClean>(t, g, prev, b0, b1, a0.x, more_a, f, a.opaque_zero, &a);
                     left -= 2;
@@ -691,11 +703,10 @@ __global__ void __maxnreg__(kRegs) ScanUniformLookKernel(const __grid_constant__
 
 // ---------------------------------------------------------------- LOOK variant, two strings per lane
 //
-// ncu on the look-ahead kernel (profiles/r02_full_glue10_lookclean.txt): a third of all stall samples sit on the LOP3 that
-// waits for the previous step's LDS, and 40 warps per SM run 2.8 % faster than 36 -- the kernel is short of independent
-// chains, and registers (48 per thread) cap the warps.  Here every lane walks TWO strings (units 2p and 2p+1 of the
+// The one-string look-ahead kernel waits mostly on the LOP3 that needs the previous step's LDS, and more warps per SM
+// run it faster -- it is short of independent chains, and registers (48 per thread) cap the warps.  Here every lane walks TWO strings (units 2p and 2p+1 of the
 // batch) step by step in turn: the second string's step fills the latency of the first one's table read, and the
-// block bookkeeping is shared.  32 data registers (two LDG.256 ping-pong sets), __maxnreg__ chosen by the launch plan.
+// block bookkeeping is shared.  32 data registers (two ping-pong sets of 32 bytes), __maxnreg__ chosen by the launch plan.
 template <bool kClean>
 __device__ __forceinline__ void LookWord2(uint32_t& ga, uint32_t wa, uint32_t bba0, uint32_t paa0, uint32_t pana, uint32_t& gb, uint32_t wb,
                                           uint32_t bbb0, uint32_t pab0, uint32_t panb, uint32_t base, const LookFilter& f)
@@ -1114,9 +1125,9 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) ScanGenericKernel
 // ---------------------------------------------------------------- long strings, split over a warp
 //
 // One string per lane makes the longest string of a batch the critical path: a 64 KiB string is 65 536 dependent
-// table reads, 3.7 ms at the 110 cycles a step takes a warp that shares its SM with 31 others -- as long as the whole
-// mixed-length benchmark batch.  Here a WARP owns one long string: lane j walks piece j of 32 (whole 32-byte blocks,
-// LDG.256 one block ahead), lane 0 from the string's true state, the others from a guess (hot id 0, the most visited
+// table reads, milliseconds for a warp that shares its SM with 31 others -- as long as the whole mixed-length
+// benchmark batch.  Here a WARP owns one long string: lane j walks piece j of 32 (whole 32-byte blocks,
+// 32-byte loads one block ahead), lane 0 from the string's true state, the others from a guess (hot id 0, the most visited
 // state).  Every lane leaves marks -- its hot id after every K blocks, in shared memory.  Then the pieces are stitched:
 // lane j's true start is lane j-1's end; a lane whose walk started from another state re-walks its piece from the true
 // one until it meets a mark (same hot id at the same position: the rest of the walk is the recorded one), replacing the
@@ -1216,10 +1227,8 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanSplitKernel(const
             uint32_t countdown = per_mark, m = 0;
             const uint32_t ahead = a.split_prefetch;
             for (uint32_t k = 0; k < trips; k += 2) {
-                // optional L2 prefetch, one per 256-byte line, `ahead` blocks in front of the walk.  ncu puts 31 % of this
-                // kernel's stall samples on the first use of a loaded word, but the prefetch measured no gain at 8..64
-                // blocks (3.09-3.12 ms with, 3.09 without): the L2::256B hint of the loads already brings the line into
-                // L2, what is exposed is the L2 -> SM trip under load.  Off by default.
+                // optional L2 prefetch, one per 256-byte line, `ahead` blocks in front of the walk.  The L2::256B hint
+                // of the loads already brings the line into L2, so this was found to gain nothing.  Off by default.
                 if (ahead && (k & 7u) == 0 && k + ahead < my_blocks)
                     PrefetchL2(piece + 32 * (size_t) (k + ahead));
                 if (k + 1 < my_blocks)
@@ -1250,7 +1259,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanSplitKernel(const
 
         // A lane whose guess was wrong walks the head of its piece again: its first block is asked for now, before the
         // stitch knows who needs it (one 32-byte L2 hit per lane and string), so that the re-walk does not begin with a
-        // bare load -- ncu had 31 % of this kernel's stall samples on the first use of a loaded word.
+        // bare load.
         uint4 head0 = make_uint4(0, 0, 0, 0), head1 = head0;
         bool head_fresh = my_blocks != 0;
         if (head_fresh)
@@ -1445,7 +1454,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanLinesKernel(const
 //
 // The lines of a newline-delimited text lie back to back, so they can be scanned where they are: the text is cut
 // into segments of a.text_segment bytes on 32-byte boundaries of the address space, lane j of a warp walks segment
-// 32 * unit + j like the uniform kernel walks a string (LDG.256, one block ahead in registers, every lane busy in
+// 32 * unit + j like the uniform kernel walks a string (32-byte loads, one block ahead in registers, every lane busy in
 // every step), and owns the lines that START inside its segment -- it runs past the segment's end until the last of
 // them is finished.  What makes this cheap:
 //   * the copy of the hot rows in shared memory maps '\n' to the start state in every row (the sink row keeps the
@@ -1709,7 +1718,7 @@ __global__ void __launch_bounds__(kBlock, kTextBlocksPerSM) ScanTextKernel(const
 // ---------------------------------------------------------------- PRIV variant
 //
 // The plain walk is bound by shared-memory wavefronts once lanes sit in different
-// rows (glued scanners: ~2.4 wavefronts per load, ncu r01).  Here the hottest rows
+// rows (glued scanners: more than two wavefronts per load).  Here the hottest rows
 // are replicated into all 32 banks: lane l reads only bank l, so every load is one
 // wavefront whatever the states and bytes are.  Layout (byte address inside the
 // private region):   [19:14] quad q   [13:7] byte b (< 128)   [6:2] lane   [1:0] row-in-quad s
@@ -2095,7 +2104,7 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) PrefixKernel(cons
         SetFull(t, s, full);
         if (!kReverse && a.uniform) {
             // Fixed-length, 32-byte aligned batch (the BASELINE configs' shape): no edge bytes, and the strings stream
-            // through registers like in the uniform scan kernel -- one LDG.256 per lane per 32 bytes, prefetched one
+            // through registers like in the uniform scan kernel -- one pair of LDG.128 per lane per 32 bytes, prefetched one
             // block ahead -- instead of the cp.async ring, whose shared-memory round trip costs half a wavefront per
             // step on the pipe that bounds the walk.
             // every lane of the warp walks the loop (its control flow holds a warp vote), also the lanes past the end
@@ -2555,7 +2564,7 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) CountKernel(const
         LaneState s;
         SetFull(t, s, full);
         if (a.uniform) {
-            // fixed-length, 32-byte aligned batch: LDG.256 ping-pong through registers, no staging ring (see PrefixKernel)
+            // fixed-length, 32-byte aligned batch: 32-byte loads ping-pong through registers, no staging ring (see PrefixKernel)
             const uint32_t len = (uint32_t) (end - p);
             if (len != 0) {
                 uint4 a0, a1, b0, b1;
@@ -2751,8 +2760,7 @@ bool LookClean()
 
 // Two strings per lane (ScanUniformLook2Kernel) is the default shape of the look-ahead variant; PIRE_B200_LOOK_ILP=1
 // selects one string per lane (ScanUniformLookKernel).  PIRE_B200_LOOK_ILP_REGS=64|72|80 picks the register budget
-// and with it the CTA shape (two CTAs of 512 / 448 / 384 threads per SM); measured 2.739 / 2.374 / 2.384 ms on the
-// glued scan (profiles/r02_experiments_notes.txt).
+// and with it the CTA shape (two CTAs of 512 / 448 / 384 threads per SM).
 int LookIlp()
 {
     static const int ilp = [] {
@@ -3221,7 +3229,7 @@ cudaError_t SplitLines(const uint8_t* d_text, uint64_t n_bytes, uint64_t* d_offs
         err = cudaMemsetAsync(d_counts, 0, 2 * sizeof(unsigned long long), stream);
     if (err == cudaSuccess) {
         uint64_t blocks = (n_bytes + 256 * 64 - 1) / (256 * 64);
-        CountNewlinesKernel<<<(unsigned) (blocks < 148 * 16 ? blocks : 148 * 16), 256, 0, stream>>>(d_text, n_bytes, d_counts);
+        CountNewlinesKernel<<<(unsigned) (blocks < GridCap(16) ? blocks : GridCap(16)), 256, 0, stream>>>(d_text, n_bytes, d_counts);
         g_launches.fetch_add(1, std::memory_order_relaxed);
         err = cudaGetLastError();
     }
@@ -3268,7 +3276,7 @@ cudaError_t LaunchSynth(const SynthParams& p, const char* d_plants, uint8_t* d_o
         return cudaSuccess;
     uint64_t total = p.n_strings * (p.string_len / 16);
     uint64_t blocks = (total + 255) / 256;
-    int grid = (int) (blocks < 148ull * 64 ? blocks : 148ull * 64);
+    int grid = (int) (blocks < GridCap(64) ? blocks : GridCap(64));
     SynthKernel<<<grid, 256, 0, stream>>>(p, d_plants, d_out);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
@@ -3289,7 +3297,7 @@ cudaError_t LaunchSynthMixedFill(uint64_t seed, uint32_t plant_every, uint64_t f
     if (n == 0)
         return cudaSuccess;
     uint64_t blocks = (n + 7) / 8;
-    SynthMixedFillKernel<<<(unsigned) (blocks < 148ull * 32 ? blocks : 148ull * 32), 256, 0, stream>>>(seed, plant_every, first, n,
+    SynthMixedFillKernel<<<(unsigned) (blocks < GridCap(32) ? blocks : GridCap(32)), 256, 0, stream>>>(seed, plant_every, first, n,
                                                                                                    d_offsets, d_out);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
@@ -3318,7 +3326,7 @@ cudaError_t LaunchAcceptGather(const uint32_t* d_table, uint32_t states, uint32_
         return cudaSuccess;
     const uint64_t total = n * words;
     const uint64_t blocks = (total + 255) / 256;
-    AcceptGatherKernel<<<(unsigned) (blocks < 148ull * 32 ? blocks : 148ull * 32), 256, 0, stream>>>(d_table, states, words, d_state_idx, n, d_out);
+    AcceptGatherKernel<<<(unsigned) (blocks < GridCap(32) ? blocks : GridCap(32)), 256, 0, stream>>>(d_table, states, words, d_state_idx, n, d_out);
     g_launches.fetch_add(1, std::memory_order_relaxed);
     return cudaGetLastError();
 }

@@ -1,5 +1,5 @@
 // scan_kernels.cuh -- launch interface between the C ABI (capi.cu) and the
-// sm_100a kernels (scan_kernels.cu).
+// sm_90a kernels (scan_kernels.cu).
 #pragma once
 
 #include <cuda_runtime.h>

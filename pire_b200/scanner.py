@@ -108,7 +108,7 @@ class Batch:
 
 
 class Scanner:
-    """A compiled multi-regexp scanner resident on one B200 (Pire::Scanner's role)."""
+    """A compiled multi-regexp scanner resident on one GPU (Pire::Scanner's role)."""
 
     def __init__(self, image, device=0):
         image = bytes(image)

@@ -13,7 +13,7 @@ for p in (HERE, ROOT):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
 
 
 class GoldenCase:
@@ -89,11 +89,21 @@ def golden():
 
 @pytest.fixture(scope="session")
 def ref():
-    """The real reference (oracle/_ref); absent when neither /root/reference nor a prebuilt copy exists."""
+    """The reference: the real one when oracle/_ref is built, else its answers stored under tests/golden (see
+    refpire.StoredRef).  PIRE_RECORD_REFERENCE=<file> records what the session asks of the real one into <file>."""
     import refpire
+    record = os.environ.get("PIRE_RECORD_REFERENCE")
     if not refpire.have_ref():
-        pytest.skip("oracle/_ref/libpire_ref.so not built (needs /root/reference)")
-    return refpire.Ref()
+        if record:
+            pytest.fail("PIRE_RECORD_REFERENCE needs oracle/_ref (oracle/build_ref.sh)")
+        yield refpire.StoredRef()
+        return
+    if not record:
+        yield refpire.Ref()
+        return
+    recorder = refpire.StoredRef(live=refpire.Ref())
+    yield recorder
+    recorder.store.save(record)
 
 
 @pytest.fixture(scope="session")

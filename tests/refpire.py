@@ -361,3 +361,240 @@ def csr(strings):
         offs[i + 1] = total
     corpus = np.frombuffer(b"".join(strings) + b"\0" * 32, dtype=np.uint8).copy()
     return corpus, offs
+
+
+# ----------------------------------------------------------------------------- the reference's answers, stored
+#
+# The tests that compare with the reference (``ref`` fixture) run without it too: every scanner image the reference
+# compiled for them and a SHA-256 of every answer it gave are kept in tests/golden/reference_answers.json.xz.  Without
+# oracle/_ref the answers are recomputed by the oracle over the stored image and must hash to what the reference
+# returned; where the oracle cannot give the reference's answer (the default scanner's LongestPrefix on 16-byte
+# boundaries, accepted-regexp lists) the answer itself is stored.  PIRE_RECORD_REFERENCE=<file> with oracle/_ref
+# built records what a test session asks of the reference into <file> (on top of the committed answers).
+
+import base64
+import hashlib
+import json
+import lzma
+
+STORED_ANSWERS = os.path.join(ROOT, "tests", "golden", "reference_answers.json.xz")
+_DATA_DIR = os.path.join(ROOT, "pire_b200", "data")
+
+
+def _sha(*parts):
+    h = hashlib.sha256()
+    for p in parts:
+        if isinstance(p, np.ndarray):
+            a = np.ascontiguousarray(p)
+            h.update(str((a.dtype.str, a.shape)).encode())
+            h.update(a.reshape(-1).view(np.uint8).data)
+        elif isinstance(p, (bytes, bytearray)):
+            h.update(bytes(p))
+        else:
+            h.update(repr(p).encode())
+        h.update(b"|")
+    return h.hexdigest()
+
+
+def _call_key(op, image_sha, corpus, offsets, params):
+    corpus = np.ascontiguousarray(corpus, dtype=np.uint8)
+    offsets = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.uint64)
+    return _sha(op, image_sha, params, corpus, b"" if offsets is None else offsets)[:24]
+
+
+def _answer_sha(arrays):
+    return _sha(*["-" if a is None else a for a in arrays])[:24]
+
+
+def _pack(a):
+    a = np.ascontiguousarray(a)
+    return {"dtype": a.dtype.str, "shape": list(a.shape), "xz": base64.b64encode(lzma.compress(a.tobytes())).decode()}
+
+
+def _unpack(d):
+    return np.frombuffer(lzma.decompress(base64.b64decode(d["xz"])), dtype=np.dtype(d["dtype"])).reshape(d["shape"]).copy()
+
+
+class AnswerStore:
+    def __init__(self, path=STORED_ANSWERS):
+        self.images, self.ops, self.calls = {}, {}, {}
+        if os.path.exists(path):
+            with open(path, "rb") as f:
+                d = json.loads(lzma.decompress(f.read()))
+            self.images, self.ops, self.calls = d["images"], d["ops"], d["calls"]
+        self._bytes = {}
+
+    def save(self, path):
+        blob = json.dumps({"images": self.images, "ops": self.ops, "calls": self.calls}, sort_keys=True, separators=(",", ":"))
+        with open(path, "wb") as f:
+            f.write(lzma.compress(blob.encode(), preset=9 | lzma.PRESET_EXTREME))
+
+    def add_image(self, image, meta):
+        sha = _sha(image)[:24]
+        if sha not in self.images:
+            entry = dict(meta)
+            for name in sorted(os.listdir(_DATA_DIR)):                # the package's own images are not stored twice
+                with open(os.path.join(_DATA_DIR, name), "rb") as f:
+                    if lzma.decompress(f.read()) == image:
+                        entry["data"] = name
+                        break
+            else:
+                entry["hex"] = image.hex()                                # the file as a whole is compressed
+            self.images[sha] = entry
+        return sha
+
+    def image(self, sha):
+        if sha not in self._bytes:
+            e = self.images[sha]
+            if "data" in e:
+                with open(os.path.join(_DATA_DIR, e["data"]), "rb") as f:
+                    self._bytes[sha] = lzma.decompress(f.read())
+            else:
+                self._bytes[sha] = bytes.fromhex(e["hex"])
+        return self._bytes[sha]
+
+
+def _oracle_answer(orc, op, corpus, offsets, fixed_len, n, kw):
+    """The oracle's answer to one of the reference's batch calls, as the tuple of arrays the reference returns."""
+    if op == "run":
+        return orc.run(corpus, offsets, fixed_len=fixed_len, n=n, begin=kw["begin"], end=kw["end"], shortcuts=True)
+    if op == "prefix":
+        return (oracle_prefix(orc, corpus, offsets, fixed_len=fixed_len, n=n, shortest=kw["shortest"],
+                              through_begin=kw["through_begin"], through_end=kw["through_end"]),)
+    if op == "suffix":
+        return (oracle_suffix(orc, corpus, offsets, fixed_len=fixed_len, n=n, shortest=kw["shortest"],
+                              through_end=kw["through_end"], through_begin=kw["through_begin"]),)
+    return oracle_count(orc, corpus, offsets, fixed_len=fixed_len, n=n, begin=kw["begin"], end=kw["end"])
+
+
+def _batch_n(corpus, offsets, fixed_len, n):
+    if offsets is not None:
+        return len(offsets) - 1 if n is None else n
+    return (len(corpus) // fixed_len if fixed_len else 0) if n is None else n
+
+
+class StoredScanner:
+    """A scanner the reference compiled, with the reference's answers: recorded from a live one (``live`` given, the
+    answers are checked against nothing and stored) or replayed through the oracle (``live`` None)."""
+
+    def __init__(self, store, sha, live=None):
+        self._store, self._sha, self._live = store, sha, live
+        meta = store.images[sha]
+        self.empty, self.size, self.letters, self.regexps = meta["empty"], meta["size"], meta["letters"], meta["regexps"]
+        self._orc = None
+
+    @property
+    def _h(self):
+        return self._live._h
+
+    def save(self):
+        return self._store.image(self._sha)
+
+    def oracle(self):
+        if self._orc is None:
+            self._orc = Oracle(self.save())
+        return self._orc
+
+    def accepted(self, state):
+        key = "accepted:%s:%d" % (self._sha, state)
+        if self._live is not None:
+            self._store.calls[key] = {"value": self._live.accepted(state)}
+        return list(self._store.calls[key]["value"])
+
+    def _batch(self, op, corpus, offsets, fixed_len, n, kw, want, live_call):
+        corpus = np.ascontiguousarray(corpus, dtype=np.uint8)
+        offsets = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.uint64)
+        n = _batch_n(corpus, offsets, fixed_len, n)
+        key = _call_key(op, self._sha, corpus, offsets, (fixed_len, n, sorted(kw.items())) + ((tuple(want),) if want else ()))
+        if self._live is not None:
+            got = live_call()
+            mine = _oracle_answer(self.oracle(), op, corpus, offsets, fixed_len, n, kw)
+            entry = {"sha": _answer_sha(got)}
+            if any(g is None for g in got):
+                entry["none"] = [i for i, g in enumerate(got) if g is None]
+            if _answer_sha(got) != _answer_sha([None if g is None else m for g, m in zip(got, mine)]):
+                entry["value"] = [None if g is None else _pack(g) for g in got]
+            self._store.calls[key] = entry
+            return got
+        if key not in self._store.calls:
+            raise KeyError("no stored reference answer for this %s call (record it with PIRE_RECORD_REFERENCE and "
+                           "oracle/_ref built)" % op)
+        entry = self._store.calls[key]
+        if "value" in entry:
+            out = tuple(None if v is None else _unpack(v) for v in entry["value"])
+        else:
+            out = _oracle_answer(self.oracle(), op, corpus, offsets, fixed_len, n, kw)
+        out = tuple(None if i in entry.get("none", ()) else a for i, a in enumerate(out))
+        assert _answer_sha(out) == entry["sha"], "the answer differs from the reference's stored one (%s)" % op
+        return out
+
+    def run(self, corpus, offsets=None, fixed_len=0, n=None, begin=True, end=True, variant=1, threads=1,
+            want=("final", "mask", "state")):
+        kw = dict(begin=bool(begin), end=bool(end), variant=variant)
+        live = lambda: self._live.run(corpus, offsets, fixed_len, n, begin, end, variant, threads, want)   # noqa: E731
+        out = self._batch("run", corpus, offsets, fixed_len, n, kw, want, live)
+        return tuple(a if name in want else None for a, name in zip(out, ("final", "mask", "state")))
+
+    def prefix(self, corpus, offsets=None, fixed_len=0, n=None, shortest=False, through_begin=False, through_end=False, variant=2):
+        kw = dict(shortest=bool(shortest), through_begin=bool(through_begin), through_end=bool(through_end), variant=variant)
+        live = lambda: (self._live.prefix(corpus, offsets, fixed_len, n, shortest, through_begin, through_end, variant),)   # noqa: E731
+        return self._batch("prefix", corpus, offsets, fixed_len, n, kw, None, live)[0]
+
+    def suffix(self, corpus, offsets=None, fixed_len=0, n=None, shortest=False, through_end=False, through_begin=False, variant=2):
+        kw = dict(shortest=bool(shortest), through_begin=bool(through_begin), through_end=bool(through_end), variant=variant)
+        live = lambda: (self._live.suffix(corpus, offsets, fixed_len, n, shortest, through_end, through_begin, variant),)   # noqa: E731
+        return self._batch("suffix", corpus, offsets, fixed_len, n, kw, None, live)[0]
+
+    def count(self, corpus, offsets=None, fixed_len=0, n=None, begin=True, end=True, threads=1):
+        kw = dict(begin=bool(begin), end=bool(end))
+        live = lambda: self._live.count(corpus, offsets, fixed_len, n, begin, end, threads)   # noqa: E731
+        return self._batch("count", corpus, offsets, fixed_len, n, kw, None, live)
+
+
+class StoredRef:
+    """``Ref``'s face over an AnswerStore: replays it, or (``live`` = a Ref) records into it."""
+
+    def __init__(self, store=None, live=None):
+        self.store = AnswerStore() if store is None else store
+        self._live = live
+
+    def _op(self, key, make):
+        key = _sha(*key)[:24]
+        if self._live is not None:
+            try:
+                sc = make()
+            except ValueError as ex:
+                self.store.ops[key] = {"error": str(ex)}
+                raise
+            meta = {"empty": bool(sc.empty), "size": int(sc.size), "regexps": int(sc.regexps),
+                    "letters": int(sc.letters) if hasattr(sc, "letters") else None}
+            self.store.ops[key] = {"image": self.store.add_image(sc.save(), meta)}
+            return StoredScanner(self.store, self.store.ops[key]["image"], sc)
+        if key not in self.store.ops:
+            raise KeyError("no stored reference scanner for this call (record it with PIRE_RECORD_REFERENCE and oracle/_ref built)")
+        entry = self.store.ops[key]
+        if "error" in entry:
+            raise ValueError(entry["error"])
+        return StoredScanner(self.store, entry["image"])
+
+    def compile(self, pattern, opts=""):
+        if isinstance(pattern, str):
+            pattern = pattern.encode("latin-1")
+        return self._op(("compile", pattern, opts), lambda: self._live.compile(pattern, opts))
+
+    def glue(self, a, b, max_size=0):
+        return self._op(("glue", a._sha, b._sha, max_size), lambda: self._live.glue(a._live, b._live, max_size))
+
+    def glue_all(self, patterns):
+        return self._op(("glue_all", [(bytes(p), o) for p, o in patterns]), lambda: self._live.glue_all(patterns))
+
+    def compile_half_final(self, pattern, opts="", mode=0):
+        if isinstance(pattern, str):
+            pattern = pattern.encode("latin-1")
+        return self._op(("compile_half_final", pattern, opts, mode), lambda: self._live.compile_half_final(pattern, opts, mode))
+
+    def glue_half_final(self, a, b, max_size=0):
+        return self._op(("glue_half_final", a._sha, b._sha, max_size), lambda: self._live.glue_half_final(a._live, b._live, max_size))
+
+    def hardware_threads(self):
+        return os.cpu_count() or 1

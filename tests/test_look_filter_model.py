@@ -3,8 +3,8 @@ synthetic text with every slot function the kernels use -- byte & 31 (LOOK), byt
 were tried and dropped (a multiplicative hash whose multiplier is searched per automaton, the LOOKH experiment, also
 with only the even positions hashed), and compares the end state of every string with the plain walk.  A filter that
 drops a byte it must not drop shows up as a mismatch here, before any GPU sees it.  The model also counts shared-memory
-wavefronts per step: the numbers DESIGN.md 8.4 / 8.8 argue from (the hashed filter is sharper -- and its kernel was
-slower all the same, profiles/r02_experiments_notes.txt)."""
+wavefronts per step: the numbers the choice of filter argues from (the hashed filter is sharper, and its kernel was
+slower all the same)."""
 import lzma
 import os
 import re

@@ -4,7 +4,7 @@ corpus (1 KiB printable-ASCII strings, 1/8 planted) for
   hf_glue10     the ten patterns as glued HalfFinalScanners (211 states; finals are rare), and
   count_words5  the five HalfFinalFsm counters of [a-z]+ (3 states; almost every byte is final),
 with a sample of every run checked against the real reference (oracle/_ref) or the oracle port.
-Usage: python tools/gpu_count_exp.py [strings]   (run on the B200 box)
+Usage: python tools/gpu_count_exp.py [strings]   (run on a GPU host)
 """
 import json
 import os

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Throughput of pire_gpu_prefix_batch (LongestPrefix / ShortestPrefix) on the configs[2] corpus.
-Usage: python tools/gpu_prefix_exp.py [strings]   (run on the B200 box)"""
+Usage: python tools/gpu_prefix_exp.py [strings]   (run on a GPU host)"""
 import json
 import os
 import sys

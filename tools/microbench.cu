@@ -34,23 +34,28 @@ __device__ __forceinline__ uint4 Ld16Alloc(const uint8_t* p)
     asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
     return v;
 }
+// sm_90 has no 256-bit load: 32 bytes of a lane are two 128-bit loads of one sector.  kL1: whether they allocate in
+// L1 (then the second half of the sector is an L1 hit; without, both halves go to L2).  The first load carries the
+// 256-byte L2 prefetch hint.
+template <bool kL1>
 __device__ __forceinline__ void Ld32(const uint8_t* p, uint4& a, uint4& b)
 {
-    asm volatile("ld.global.nc.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(p));
-}
-__device__ __forceinline__ void Ld32Hint(const uint8_t* p, uint4& a, uint4& b)
-{
-    asm volatile("ld.global.nc.L1::no_allocate.L2::256B.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
-                 : "l"(p));
+    if (kL1)
+        asm volatile("ld.global.nc.L2::256B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                     "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
+                     : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
+                     : "l"(p));
+    else
+        asm volatile("ld.global.nc.L1::no_allocate.L2::256B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                     "ld.global.nc.L1::no_allocate.v4.u32 {%4,%5,%6,%7}, [%8+16];"
+                     : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
+                     : "l"(p));
 }
 __device__ __forceinline__ uint32_t Fold(uint4 v) { return v.x ^ v.y ^ v.z ^ v.w; }
 
 // mode 0: LDG.128 no_allocate, depth 1   mode 1: LDG.128 allocate (second half of the sector hits L1)
-// mode 2: LDG.256                        mode 3: LDG.256 + L2::256B prefetch hint
-// mode 4: 2 x LDG.256 in flight          mode 5: coalesced contiguous LDG.128 (upper bound)
+// mode 2: 2 x LDG.128 per 32 B, no_allocate   mode 3: 2 x LDG.128 per 32 B, allocating in L1
+// mode 4: mode 3 with two 32-byte blocks in flight   mode 5: coalesced contiguous LDG.128 (upper bound)
 template <int kMode>
 __global__ void __launch_bounds__(512) LoadKernel(const uint8_t* corpus, uint64_t n, uint32_t len, uint32_t* out)
 {
@@ -74,9 +79,9 @@ __global__ void __launch_bounds__(512) LoadKernel(const uint8_t* corpus, uint64_
                 acc ^= Fold(cur);
             } else if (kMode == 2 || kMode == 3) {
                 uint4 a0, a1, b0, b1;
-                if (kMode == 2) Ld32(p, a0, a1); else Ld32Hint(p, a0, a1);
+                Ld32<kMode == 3>(p, a0, a1);
                 for (uint32_t off = 32; off < len; off += 32) {
-                    if (kMode == 2) Ld32(p + off, b0, b1); else Ld32Hint(p + off, b0, b1);
+                    Ld32<kMode == 3>(p + off, b0, b1);
                     acc ^= Fold(a0) ^ Fold(a1);
                     a0 = b0;
                     a1 = b1;
@@ -84,10 +89,10 @@ __global__ void __launch_bounds__(512) LoadKernel(const uint8_t* corpus, uint64_
                 acc ^= Fold(a0) ^ Fold(a1);
             } else {
                 uint4 a0, a1, b0, b1, c0, c1;
-                Ld32(p, a0, a1);
-                Ld32(p + 32, b0, b1);
+                Ld32<true>(p, a0, a1);
+                Ld32<true>(p + 32, b0, b1);
                 for (uint32_t off = 64; off < len; off += 32) {
-                    Ld32(p + off, c0, c1);
+                    Ld32<true>(p + off, c0, c1);
                     acc ^= Fold(a0) ^ Fold(a1);
                     a0 = b0; a1 = b1; b0 = c0; b1 = c1;
                 }
@@ -140,10 +145,12 @@ void RunPipe(const char* name, uint32_t* out)
     CK(cudaEventSynchronize(e1));
     float ms;
     CK(cudaEventElapsedTime(&ms, e0, e1));
-    // warp-level ops of each kind per clock per SM, assuming 1965 MHz
+    // warp-level ops of each kind per clock per SM, at the device's maximum SM clock
+    int khz = 0;
+    CK(cudaDeviceGetAttribute(&khz, cudaDevAttrClockRate, 0));
     double ops = (double) iters * 8 * 48;        // per SM: 48 warps
     std::printf("{\"bench\": \"pipe\", \"mode\": \"%s\", \"ms\": %.3f, \"warp_ops_per_clk_per_sm_each\": %.3f}\n", name, ms,
-                ops / (ms * 1e-3 * 1.965e9));
+                ops / (ms * 1e-3 * khz * 1e3));
     std::fflush(stdout);
 }
 
@@ -194,9 +201,9 @@ int main(int argc, char** argv)
         Run<5>("coalesced_ldg128", d, n, len, out, tps);
         Run<0>("lane_ldg128_noalloc", d, n, len, out, tps);
         Run<1>("lane_ldg128_l1", d, n, len, out, tps);
-        Run<2>("lane_ldg256", d, n, len, out, tps);
-        Run<3>("lane_ldg256_l2hint", d, n, len, out, tps);
-        Run<4>("lane_ldg256_depth2", d, n, len, out, tps);
+        Run<2>("lane_2xldg128_noalloc", d, n, len, out, tps);
+        Run<3>("lane_2xldg128_l1", d, n, len, out, tps);
+        Run<4>("lane_2xldg128_l1_depth2", d, n, len, out, tps);
     }
     return 0;
 }

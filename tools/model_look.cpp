@@ -30,7 +30,7 @@ using namespace pire_b200;
 // `address` = the table's shared-memory address, which the walk adds to every byte anyway.  FoldLookFilter folds an exact
 // set (bit b & 31 of exact[b >> 5]) onto those slots; ChooseLookMul searches the multiplier that lets the fewest bytes
 // pass (printable ASCII weighted 8:1), over slot widths of 1 to 11 byte values and 32 phases.  The kernel built on it was
-// bit-exact and slower (IMAD.HI issues at a quarter of the rate): profiles/r02_experiments_notes.txt.
+// bit-exact and slower (IMAD.HI issues at a quarter of the rate).
 static uint32_t FoldLookFilter(const uint32_t exact[8], uint32_t table_address, uint32_t mul)
 {
     uint32_t filter = 0;

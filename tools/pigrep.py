@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""pigrep on a B200: the reference's samples/pigrep/pigrep.cpp with the per-line loop
+"""pigrep on the GPU: the reference's samples/pigrep/pigrep.cpp with the per-line loop
 (std::getline + Runner(sc).Begin().Run(line).End()) moved to the device.
 
     python tools/pigrep.py --scanner patterns.pire file [file ...]     # precompiled Scanner::Save() image

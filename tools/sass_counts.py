@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Per-kernel SASS evidence for profiles/: which of the mnemonics the design relies on each kernel of
+"""Per-kernel SASS evidence: which of the mnemonics the design relies on each kernel of
 pire_b200/libpire_b200.so really contains (cuobjdump -sass; no GPU needed).
 
-    python tools/sass_counts.py > profiles/r02_sass_counts.txt
+    python tools/sass_counts.py > sass_counts.txt
 """
 import collections
 import os
@@ -16,8 +16,7 @@ WATCH = [
     ("UBLKCP", r"\bUBLKCP"),                     # cp.async.bulk (1-D TMA): table staging
     ("SYNCS", r"\bSYNCS"),                       # mbarrier arrive / try_wait
     ("LDGSTS", r"\bLDGSTS"),                     # cp.async 16 B: staging ring of the CSR kernels
-    ("LDG.256", r"\bLDG\.E\.[A-Z0-9.]*256"),     # streaming 32-byte loads of the uniform kernels
-    ("LDG.128", r"\bLDG\.E\.[A-Z0-9.]*128"),
+    ("LDG.128", r"\bLDG\.E\.[A-Z0-9.]*128"),       # streaming loads of the uniform kernels, two per 32 bytes
     ("LDS.U8", r"\bLDS\.U8"),                    # the table walk
     ("@P LDS.U8", r"@!?P\d\s+LDS\.U8"),          # predicated walk (exit filter / look-ahead)
     ("LDS.128", r"\bLDS\.128"),
