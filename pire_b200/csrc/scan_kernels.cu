@@ -161,9 +161,14 @@ __device__ __forceinline__ void LoadStream32P(const uint8_t* p, uint4& a, uint4&
                  : "l"(p));
 }
 
+// The uniform kernels' load: the first half carries the 128-byte L2 prefetch-size hint, so an L2 miss fetches the
+// sector's whole 128-byte line and HBM serves whole lines instead of scattered 32-byte sectors (the three other
+// sectors of the line are the lane's next three blocks).  The lines of every string in progress stay in L2: at most
+// 132 SMs x 48 warps x 32 strings x 128 B = 26 MB on an H100, of its 50 MB.  The 256-byte hint would take twice that,
+// and the two-strings-per-lane kernel (29 MB at 128 B) measured slower with it.
 __device__ __forceinline__ void LoadStream32(const uint8_t* p, uint4& a, uint4& b)
 {
-    asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+    asm volatile("ld.global.nc.L2::128B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
                  "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
                  : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w)
                  : "l"(p));

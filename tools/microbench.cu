@@ -5,7 +5,13 @@
 // (shared-memory wavefronts) or to the loads (L1TEX tag stage: 32 distinct
 // lines per warp-wide request).  Not part of the product library.
 //
+// The "flagship" rows run at the glued scan's shapes: the register kernel's residency (two CTAs of 448 threads, 28
+// warps per SM) with two strings per lane (units 2p and 2p+1 of a pair, one 32-byte block of each in flight), and a
+// TMA-staged alternative (one CTA of 1024 threads per SM, a per-warp ring of 64-row x 32-byte tiles read with
+// LDS.128), the shape a shared-memory-fed walk would need beside a 75 KB hot table.
+//
 //   microbench [GiB=4] [string_len=1024]
+#include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <cstdint>
@@ -52,6 +58,119 @@ __device__ __forceinline__ void Ld32(const uint8_t* p, uint4& a, uint4& b)
                      : "l"(p));
 }
 __device__ __forceinline__ uint32_t Fold(uint4 v) { return v.x ^ v.y ^ v.z ^ v.w; }
+
+// The shipped load of ScanUniformLook2Kernel: two LDG.128 of one sector, both allocating in L1.  kL2 = 0, 64, 128 or
+// 256: the first load carries the L2 prefetch-size hint of that many bytes.
+template <int kL2>
+__device__ __forceinline__ void Ld32Pair(const uint8_t* p, uint4& a, uint4& b)
+{
+    if (kL2 == 64)
+        asm volatile("ld.global.nc.L2::64B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                     "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
+                     : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
+    else if (kL2 == 128)
+        asm volatile("ld.global.nc.L2::128B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                     "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
+                     : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
+    else if (kL2 == 256)
+        asm volatile("ld.global.nc.L2::256B.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                     "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
+                     : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
+    else
+        asm volatile("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+                     "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
+                     : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
+}
+
+// Two strings per lane (rows 64p + lane and 64p + 32 + lane), the next 32-byte block of both in flight while the
+// current one is folded: the input side of ScanUniformLook2Kernel without the walk.
+template <int kL2>
+__global__ void __launch_bounds__(448) LoadPairKernel(const uint8_t* corpus, uint64_t n, uint32_t len, uint32_t* out)
+{
+    const uint64_t warps = (uint64_t) gridDim.x * (blockDim.x / 32);
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t acc = 0;
+    for (uint64_t pair = (uint64_t) blockIdx.x * (blockDim.x / 32) + (threadIdx.x >> 5); pair < n / 64; pair += warps) {
+        const uint8_t* pa = corpus + (pair * 64 + lane) * (uint64_t) len;
+        const uint8_t* pb = pa + 32 * (uint64_t) len;
+        uint4 a0, a1, b0, b1, c0, c1, d0, d1;
+        Ld32Pair<kL2>(pa, a0, a1);
+        Ld32Pair<kL2>(pb, b0, b1);
+        for (uint32_t off = 32; off < len; off += 32) {
+            Ld32Pair<kL2>(pa + off, c0, c1);
+            Ld32Pair<kL2>(pb + off, d0, d1);
+            acc ^= Fold(a0) ^ Fold(a1) ^ Fold(b0) ^ Fold(b1);
+            a0 = c0; a1 = c1; b0 = d0; b1 = d1;
+        }
+        acc ^= Fold(a0) ^ Fold(a1) ^ Fold(b0) ^ Fold(b1);
+    }
+    if (acc == 0x12345678u)
+        out[0] = acc;
+}
+
+// ---- TMA tiles: one CTA of 32 warps per SM, each warp a ring of kStages tiles of 64 rows x 32 bytes (SWIZZLE_32B)
+constexpr uint32_t kTileBytes = 64 * 32;
+
+__device__ __forceinline__ void MbarWait(uint32_t bar, uint32_t parity)
+{
+    asm volatile("{\n.reg .pred p;\nW_%=:\nmbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n@!p bra W_%=;\n}\n" ::"r"(bar),
+                 "r"(parity) : "memory");
+}
+
+__device__ __forceinline__ void IssueTile(uint32_t dst, uint32_t bar, const CUtensorMap* tm, uint32_t x, uint32_t y)
+{
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "n"(kTileBytes) : "memory");
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
+                 "l"(tm), "r"(x), "r"(y), "r"(bar)
+                 : "memory");
+}
+
+template <int kStages>
+__global__ void __launch_bounds__(1024, 1) TmaTileKernel(const __grid_constant__ CUtensorMap tm, uint64_t n, uint32_t len, uint32_t* out)
+{
+    extern __shared__ __align__(1024) uint8_t tiles[];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t warps = gridDim.x * (blockDim.x / 32);
+    const uint32_t ring = (uint32_t) __cvta_generic_to_shared(tiles) + warp * kStages * kTileBytes;
+    const uint32_t bars = (uint32_t) __cvta_generic_to_shared(tiles) + 32 * kStages * kTileBytes + warp * kStages * 8;
+    if (ring & 1023)
+        __trap();
+    if (lane == 0) {
+        for (int s = 0; s < kStages; ++s)
+            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bars + 8 * s) : "memory");
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncwarp();
+    const uint32_t chunks = len / 32, pairs = (uint32_t) (n / 64);
+    const uint32_t first = blockIdx.x * (blockDim.x / 32) + warp;
+    const uint32_t mine = first < pairs ? (pairs - first + warps - 1) / warps * chunks : 0;    // (pair, chunk) items
+    for (uint32_t k = 0; k < kStages && k < mine; ++k)
+        if (lane == 0)
+            IssueTile(ring + k * kTileBytes, bars + 8 * k, &tm, (k % chunks) * 32, (first + k / chunks * warps) * 64);
+    // 32B swizzle: the 16-byte half j of row r sits at r * 32 + 16 * (j ^ ((r >> 2) & 1))
+    const uint32_t row = lane * 32, swz = (lane >> 2) & 1;
+    uint32_t acc = 0;
+    for (uint32_t k = 0; k < mine; ++k) {
+        const uint32_t slot = k % kStages;
+        MbarWait(bars + 8 * slot, (k / kStages) & 1);
+        const uint32_t at = ring + slot * kTileBytes + row;
+        uint4 v[4];
+        for (int h = 0; h < 4; ++h)
+            asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];"
+                         : "=r"(v[h].x), "=r"(v[h].y), "=r"(v[h].z), "=r"(v[h].w)
+                         : "r"(at + (h >> 1) * 1024 + 16 * ((h & 1) ^ swz))
+                         : "memory");
+        acc ^= Fold(v[0]) ^ Fold(v[1]) ^ Fold(v[2]) ^ Fold(v[3]);
+        __syncwarp();
+        const uint32_t next = k + kStages;
+        if (lane == 0 && next < mine) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            IssueTile(ring + slot * kTileBytes, bars + 8 * slot, &tm, (next % chunks) * 32, (first + next / chunks * warps) * 64);
+        }
+    }
+    if (acc == 0x12345678u)
+        out[0] = acc;
+}
 
 // mode 0: LDG.128 no_allocate, depth 1   mode 1: LDG.128 allocate (second half of the sector hits L1)
 // mode 2: 2 x LDG.128 per 32 B, no_allocate   mode 3: 2 x LDG.128 per 32 B, allocating in L1
@@ -182,11 +301,70 @@ void Run(const char* name, const uint8_t* d, uint64_t n, uint32_t len, uint32_t*
     std::fflush(stdout);
 }
 
+void Report(const char* name, int threads_per_sm, uint64_t n, uint32_t len, float best)
+{
+    std::printf("{\"bench\": \"load\", \"mode\": \"%s\", \"threads_per_sm\": %d, \"GBps\": %.1f, \"ms\": %.3f}\n", name,
+                threads_per_sm, (double) n * len / best / 1e6, best);
+    std::fflush(stdout);
+}
+
+template <typename Launch>
+float Best(Launch launch)
+{
+    cudaEvent_t e0, e1;
+    CK(cudaEventCreate(&e0));
+    CK(cudaEventCreate(&e1));
+    for (int i = 0; i < 2; ++i)
+        launch();
+    CK(cudaGetLastError());
+    CK(cudaDeviceSynchronize());
+    float best = 1e30f;
+    for (int rep = 0; rep < 5; ++rep) {
+        CK(cudaEventRecord(e0));
+        launch();
+        CK(cudaEventRecord(e1));
+        CK(cudaEventSynchronize(e1));
+        float ms;
+        CK(cudaEventElapsedTime(&ms, e0, e1));
+        best = ms < best ? ms : best;
+    }
+    return best;
+}
+
+template <int kStages>
+void RunTma(const char* name, const uint8_t* d, uint64_t n, uint32_t len, uint32_t* out)
+{
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+    using Encode = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
+                                const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    void* fn = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    CK(cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &fn, 12000, cudaEnableDefault, &q));
+    if (!fn || q != cudaDriverEntryPointSuccess) {
+        std::fprintf(stderr, "cuTensorMapEncodeTiled unavailable\n");
+        std::exit(1);
+    }
+    alignas(64) CUtensorMap tm;
+    const cuuint64_t dims[2] = {len, n}, strides[1] = {len};
+    const cuuint32_t box[2] = {32, 64}, estr[2] = {1, 1};
+    CUresult r = reinterpret_cast<Encode>(fn)(&tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<uint8_t*>(d), dims, strides, box, estr,
+                                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_32B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) {
+        std::fprintf(stderr, "cuTensorMapEncodeTiled: %d\n", (int) r);
+        std::exit(1);
+    }
+    const size_t smem = (size_t) 32 * kStages * kTileBytes + 32 * kStages * 8;
+    CK(cudaFuncSetAttribute(TmaTileKernel<kStages>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+    Report(name, 1024, n, len, Best([&] { TmaTileKernel<kStages><<<sms, 1024, smem>>>(tm, n, len, out); }));
+}
+
 int main(int argc, char** argv)
 {
     const double gib = argc > 1 ? std::atof(argv[1]) : 4.0;
     const uint32_t len = argc > 2 ? (uint32_t) std::atoi(argv[2]) : 1024;
-    const uint64_t n = (uint64_t) (gib * (1ull << 30) / len) / 32 * 32;
+    const uint64_t n = (uint64_t) (gib * (1ull << 30) / len) / 64 * 64;
     uint8_t* d;
     uint32_t* out;
     CK(cudaMalloc(&d, n * len));
@@ -197,6 +375,18 @@ int main(int argc, char** argv)
     RunPipe<3>("lds_and_shfl", out);
     if (argc > 3)
         return 0;
+    {
+        int sms = 0;
+        CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+        // the flagship's shapes first, each next to the coalesced bound at the same residency
+        Run<5>("coalesced_ldg128", d, n, len, out, 1024);
+        Report("flagship_lane_2xldg128_l1_two_strings", 896, n, len, Best([&] { LoadPairKernel<0><<<sms * 2, 448>>>(d, n, len, out); }));
+        Report("two_strings_l2_64B", 896, n, len, Best([&] { LoadPairKernel<64><<<sms * 2, 448>>>(d, n, len, out); }));
+        Report("two_strings_l2_128B", 896, n, len, Best([&] { LoadPairKernel<128><<<sms * 2, 448>>>(d, n, len, out); }));
+        Report("two_strings_l2_256B", 896, n, len, Best([&] { LoadPairKernel<256><<<sms * 2, 448>>>(d, n, len, out); }));
+        RunTma<2>("flagship_tma_tile_64x32_swz32_2stages", d, n, len, out);
+        RunTma<3>("tma_tile_64x32_swz32_3stages", d, n, len, out);
+    }
     for (int tps : {1024, 1536, 2048}) {
         Run<5>("coalesced_ldg128", d, n, len, out, tps);
         Run<0>("lane_ldg128_noalloc", d, n, len, out, tps);
