@@ -197,6 +197,65 @@ private:
 
 inline BatchRunner Runner(const Scanner& sc) { return BatchRunner(sc); }     // run.h:388-389
 
+// Counterpart of Pire::RunHelper (run.h:365-392) for ONE string resident in HBM, scanned by the whole GPU
+// (pire_gpu_run_string).  Run() may be called many times: the pieces are scanned as one string, the state carried in
+// the caller-owned device word d_state (StateIndex, reference numbering), so chained calls do not synchronise.  Every
+// call is asynchronous on `stream`; after End() the caller's device words hold the results (d_match_bits[0] bit 0 =
+// Final(), d_accept_masks[0], *d_state), as pire_gpu_run_batch writes them for n = 1.
+//     StringRunner r(gsc, d_state);                                // Runner(sc): from Initialize()
+//     StringRunner r(gsc, StringRunner::From(d_start), d_state);   // Runner(sc, st): st in the device word d_start
+//     r.Begin().Run(d_a, n_a).Run(d_b, n_b).End();
+// The start word is tagged (From) so that it can never be taken for d_state or an output: every untagged call starts
+// from Initialize().
+class StringRunner {
+public:
+    // the device word holding the StateIndex a run starts from (Runner(sc, st), run.h:391-392)
+    struct StartWord {
+        explicit StartWord(const uint32_t* d_word) : Word(d_word) {}
+        const uint32_t* Word;
+    };
+    static StartWord From(const uint32_t* d_start) { return StartWord(d_start); }
+
+    StringRunner(const Scanner& sc, uint32_t* d_state, uint32_t* d_match_bits = nullptr, uint32_t* d_accept_masks = nullptr,
+                 void* stream = nullptr)
+        : Sc(&sc), Start(nullptr), State(d_state), Bits(d_match_bits), Masks(d_accept_masks), Stream(stream), Flags(0), Ran(false)
+    {
+        if (!d_state)
+            throw Error(PIRE_GPU_EINVAL, "StringRunner needs a device word for its state");
+    }
+    // start.Word may be d_state: the state is then updated in place
+    StringRunner(const Scanner& sc, StartWord start, uint32_t* d_state, uint32_t* d_match_bits = nullptr,
+                 uint32_t* d_accept_masks = nullptr, void* stream = nullptr)
+        : StringRunner(sc, d_state, d_match_bits, d_accept_masks, stream)
+    {
+        if (!start.Word)
+            throw Error(PIRE_GPU_EINVAL, "StringRunner::From needs a device word");
+        Start = start.Word;
+    }
+
+    StringRunner& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }                   // run.h:375, with the next launch
+    StringRunner& Run(const uint8_t* d_text, uint64_t n) { Launch(d_text, n, 0); return *this; }   // run.h:372-373
+    StringRunner& End() { Launch(nullptr, 0, PIRE_GPU_RUN_END); return *this; }             // run.h:376
+
+private:
+    void Launch(const uint8_t* d_text, uint64_t n, unsigned end)
+    {
+        Check(pire_gpu_run_string(Sc->Raw(), d_text, n, Flags | end, Ran ? State : Start, Bits, Masks, State, Stream),
+              "pire_gpu_run_string");
+        Flags = 0;
+        Ran = true;
+    }
+
+    const Scanner* Sc;
+    const uint32_t* Start;
+    uint32_t* State;
+    uint32_t* Bits;
+    uint32_t* Masks;
+    void* Stream;
+    unsigned Flags;
+    bool Ran;
+};
+
 // AcceptedRegexps for scanners with more than 32 regexps: rows of AcceptWords(sc) words, bit r of row i set iff
 // regexp r is accepted by the state string i stopped in (d_state_idx from BatchRunner::Launch).
 inline uint32_t AcceptWords(const Scanner& sc) { return pire_gpu_accept_words(sc.Raw()); }

@@ -49,6 +49,7 @@ void DeviceTables::Free()
     cudaFree(acc_ids);
     cudaFree(weights);
     cudaFree(accept_wide);
+    cudaFree(new_of_old);
     *this = DeviceTables();
 }
 
@@ -129,6 +130,10 @@ int Upload(pire_gpu_scanner* sc)
         CUDA_TRY(cudaMalloc(&d.accept_wide, wide.size() * 4));
         CUDA_TRY(cudaMemcpy(d.accept_wide, wide.data(), wide.size() * 4, cudaMemcpyHostToDevice));
     }
+    // tuning renumbers the states: the map is rebuilt with the other tables
+    CUDA_TRY(cudaMalloc(&d.new_of_old, t.new_of_old.size() * 4 + 4));
+    if (!t.new_of_old.empty())
+        CUDA_TRY(cudaMemcpy(d.new_of_old, t.new_of_old.data(), t.new_of_old.size() * 4, cudaMemcpyHostToDevice));
     sc->priv_ok = false;
     for (int v = kVariantPlain; v <= kVariantLook1; ++v)
         for (int u = 0; u < 2; ++u) {
@@ -570,6 +575,35 @@ static int RunCsr(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uin
         cudaFreeAsync(counter, st);
     if (ce != cudaSuccess)
         return FailCuda(ce, "pire_gpu_run_batch (CSR)");
+    return PIRE_GPU_OK;
+}
+
+int pire_gpu_run_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uint64_t n_bytes, uint32_t flags,
+                        const uint32_t* d_start, uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx,
+                        void* stream)
+{
+    int rc = CheckRunnable(sc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_run_string takes PIRE_GPU_RUN_BEGIN and PIRE_GPU_RUN_END only");
+    if (!d_text && n_bytes)
+        return Fail(PIRE_GPU_EINVAL, "null text with n_bytes > 0");
+    CUDA_TRY(cudaSetDevice(sc->device));
+    ScanArgs a;
+    FillArgs(sc, &a, d_text, nullptr, n_bytes, 1, flags);
+    a.start_idx = d_start;
+    a.new_of_old = sc->dev.new_of_old;
+    a.states = sc->tab.states;
+    a.with_begin = (flags & PIRE_GPU_RUN_BEGIN) ? 1 : 0;
+    a.begin_class = sc->tab.begin_class;
+    a.match_bits = d_match_bits;
+    a.accept_masks = d_accept_masks;
+    a.state_idx = d_state_idx;
+    uint32_t variant = ResolveVariant(sc, false);
+    if (variant == PIRE_GPU_VARIANT_PRIV)
+        variant = PIRE_GPU_VARIANT_PLAIN;
+    CUDA_TRY(LaunchString(a, (int) variant, sc->device, static_cast<cudaStream_t>(stream)));
     return PIRE_GPU_OK;
 }
 

@@ -40,6 +40,7 @@ struct DeviceTables {
     uint32_t* acc_ids = nullptr;
     uint64_t* weights = nullptr;
     uint32_t* accept_wide = nullptr;     // [states x accept_words], reference numbering: AcceptedRegexps as a bit set
+    uint32_t* new_of_old = nullptr;      // [states]: reference numbering -> new (start states given by the caller)
     size_t full_bytes = 0;
 
     void Free();

@@ -68,6 +68,12 @@ struct ScanArgs {
     const uint64_t* weights;     // [states * count_words] packed per-state increments, or null
     uint32_t count_words;        // 0 = walk the accept lists, 1..2 = packed increments
     uint32_t count_always;       // final states are frequent: count every chunk, skip the look-ahead pass
+    // one string over the grid (pire_gpu_run_string): corpus, fixed_len = its bytes
+    const uint32_t* start_idx;   // the start as a StateIndex (reference numbering) in device memory, or null: `start`
+    const uint32_t* new_of_old;  // [states]: reference numbering -> new
+    uint32_t states;             // Size(): a start_idx at or above it is out of range
+    uint32_t* string_ends;       // scratch: 2 x warps of the grid, each warp's end state per stitching round
+    unsigned int* string_rounds; // scratch: 3 counters of changed warps, zeroed before the launch
 };
 
 struct LaunchPlan {
@@ -87,6 +93,9 @@ cudaError_t LaunchScan(const ScanArgs& a, int variant, bool uniform, const Launc
 cudaError_t LaunchLines(const ScanArgs& a, int variant, int device, cudaStream_t stream);
 // length-ordered CSR batches: the leading long strings, one per warp; sets *a.split_count, which the generic launch honours
 cudaError_t LaunchSplit(const ScanArgs& a, int variant, int device, cudaStream_t stream);
+// one string (a.corpus, a.fixed_len bytes) over the whole grid, cooperatively launched; a.with_begin / a.begin_class
+// step BeginMark from *a.start_idx when that is given
+cudaError_t LaunchString(const ScanArgs& a, int variant, int device, cudaStream_t stream);
 cudaError_t LaunchVisitCount(const ScanArgs& a, cudaStream_t stream);
 // prefix (left to right) or suffix (right to left) scan; a.with_begin/begin_class name the mark stepped first,
 // a.through_end/end_class the mark stepped last

@@ -313,6 +313,87 @@ class RunHelper:
         return self.Sc.AcceptedRegexps(int(self.States()[i]))
 
 
+class StringRunner:
+    """Pire::RunHelper (run.h:365-392) for ONE string resident in HBM, scanned by the whole GPU
+    (pire_gpu_run_string).  ``Run(text)`` may be called many times: the texts are scanned as one string, the state
+    carried from call to call in a device word, so chained calls do not synchronise (a stream arriving in chunks).
+    ``state`` = a StateIndex to start from (``Runner(sc, st)``, run.h:391-392), None = Initialize().  Every ``Run()``
+    launches at once on the current stream, so a buffer may be refilled behind it in stream order; ``Begin()`` is
+    folded into the first launch, ``End()`` is a launch of its own.  Results (``State()``, ``Final()``,
+    ``AcceptedRegexps()``, ``bool``) synchronise.
+
+    To tune the shared-memory rows for a long string, pass a fixed-length view of it to ``Scanner.Tune``, e.g.
+    ``sc.Tune(Batch(text[: len(text) // 4096 * 4096], fixed_len=4096))``."""
+
+    def __init__(self, sc, state=None):
+        self.Sc = sc
+        self._start = None if state is None else int(state)
+        self._words = None         # device: [StateIndex, match word, accept mask]
+        self._begin = False
+        self._ran = False          # a launch has written the state word
+
+    def Begin(self):
+        if self._ran:
+            raise ValueError("Begin() must precede Run()")
+        self._begin = True
+        return self
+
+    def Run(self, text):
+        torch = _torch()
+        if text.dtype != torch.uint8 or not text.is_cuda or not text.is_contiguous() or text.device.index != self.Sc.device:
+            raise ValueError("text must be a contiguous uint8 CUDA tensor on the scanner's device")
+        self._launch(text, 0)
+        return self
+
+    def End(self):
+        self._launch(None, N.RUN_END)
+        return self
+
+    def _launch(self, text, flags):
+        if self._begin:
+            flags |= N.RUN_BEGIN
+            self._begin = False
+        start = stream = None
+        if self.Sc.device >= 0:
+            torch = _torch()
+            dev = torch.device("cuda", self.Sc.device)
+            if self._words is None:
+                self._words = torch.empty(3, dtype=torch.int32, device=dev)
+                if self._start is not None:
+                    word = self._start & 0xFFFFFFFF
+                    self._words[0] = word - (1 << 32) if word >= (1 << 31) else word
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            if self._ran or self._start is not None:
+                start = self._words.data_ptr()
+        ptr = None if self._words is None else self._words.data_ptr()
+        N.check(N.lib.pire_gpu_run_string(self.Sc._h, None if text is None else text.data_ptr(), 0 if text is None else text.numel(),
+                                          flags, start, None if ptr is None else ptr + 4, None if ptr is None else ptr + 8, ptr,
+                                          stream), "pire_gpu_run_string")
+        self._ran = True
+
+    def _results(self):
+        if not self._ran:
+            self._launch(None, 0)          # nothing run yet: the start state itself (after Begin() if it was asked for)
+        return self._words.cpu().numpy().view(np.uint32)
+
+    def State(self):
+        """StateIndex() of the state reached (reference numbering); 0xFFFFFFFF for a start outside the scanner."""
+        return int(self._results()[0])
+
+    def Final(self):
+        return bool(self._results()[1] & 1)
+
+    def __bool__(self):
+        return self.Final()
+
+    def AcceptMask(self):
+        """AcceptedRegexps as a bit mask of the ids below 32."""
+        return int(self._results()[2])
+
+    def AcceptedRegexps(self):
+        return self.Sc.AcceptedRegexps(self.State())
+
+
 def Runner(sc):
     """Pire::Runner(sc) (run.h:388-389)."""
     return RunHelper(sc)
