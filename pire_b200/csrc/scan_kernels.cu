@@ -21,7 +21,8 @@
 //     so fewer lanes hit the banks and the load costs fewer wavefronts.
 //   * LOOK variant (the glued benchmark scan): the filter looks one byte further -- a resting
 //     lane reads the table only if this byte and the next both pass -- in 5.5 instructions per
-//     byte (LookProbe / LookStep), two strings per lane (ScanUniformLook2Kernel).
+//     byte (LookProbe / LookStep), two strings per lane (ScanUniformLookRingKernel, fed from a per-lane cp.async ring
+//     with two blocks of each string in flight; ScanUniformLook2Kernel, fed from registers).
 //   * Input bytes: each lane streams its own string: 32-byte read-only loads (two
 //     LDG.128 of one sector, the second an L1 hit), one ahead in a register ping-pong (uniform kernels,
 //     two LDG.128 per 32 bytes), or a four-deep cp.async ring of 16-byte chunks in shared memory
@@ -735,10 +736,13 @@ __device__ __forceinline__ void LookWord2(uint32_t& ga, uint32_t wa, uint32_t bb
     LookStep<kClean>(gb, bbb3, pab3, panb);
 }
 
-template <bool kClean>
-__device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uint32_t& preva, const uint4& a0, const uint4& a1, uint32_t nexta,
-                                              uint32_t& gb, uint32_t& prevb, const uint4& b0, const uint4& b1, uint32_t nextb, bool more,
-                                              const LookFilter& f, uint32_t opaque_zero, const ScanArgs* args)
+// `late(ga, gb, nexta, nextb)` fetches the first words of the blocks that follow, after the walk of the block's first 28
+// bytes (see LookBlock32): from registers loaded a block ahead (ScanUniformLook2Kernel) or from the ring in shared memory
+// (ScanUniformLookRingKernel).
+template <bool kClean, typename Late>
+__device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uint32_t& preva, const uint4& a0, const uint4& a1,
+                                              uint32_t& gb, uint32_t& prevb, const uint4& b0, const uint4& b1, bool more,
+                                              const LookFilter& f, Late late, const ScanArgs* args)
 {
     preva = ga == t.H ? preva : ga;
     prevb = gb == t.H ? prevb : gb;
@@ -767,8 +771,8 @@ __device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uin
     LookProbe<false, 0, kClean>(b1.w, t.base, f, bnb, pnb);
     LookWord2<kClean>(ga, a1.z, bba, paa, pna, gb, b1.z, bbb, pab, pnb, t.base, f);
     // the words after the blocks are still on their way from HBM: their probes stay behind the walk (see LookBlock32)
-    const uint32_t latea = nexta + ga * opaque_zero;
-    const uint32_t lateb = nextb + gb * opaque_zero;
+    uint32_t latea, lateb;
+    late(ga, gb, latea, lateb);
     LookProbe<false, 0, kClean>(latea, t.base, f, bba, paa);
     LookProbe<false, 0, kClean>(lateb, t.base, f, bbb, pab);
     LookWord2<kClean>(ga, a1.w, bna, pna, more ? paa : 0x80000000u, gb, b1.w, bnb, pnb, more ? pab : 0x80000000u, t.base, f);
@@ -780,6 +784,21 @@ __device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uin
         prevb = ReplayBlock32(args, prevb, b0, b1);
         gb = prevb < t.H ? prevb : t.H;
     }
+}
+
+// The next words are in registers, loaded a block ahead: they are made to depend on the walk itself -- plus g times a
+// kernel argument that is always zero -- so that their probes stay behind it.
+template <bool kClean>
+__device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uint32_t& preva, const uint4& a0, const uint4& a1, uint32_t nexta,
+                                              uint32_t& gb, uint32_t& prevb, const uint4& b0, const uint4& b1, uint32_t nextb, bool more,
+                                              const LookFilter& f, uint32_t opaque_zero, const ScanArgs* args)
+{
+    LookBlock32x2<kClean>(t, ga, preva, a0, a1, gb, prevb, b0, b1, more, f,
+                          [=](uint32_t ga, uint32_t gb, uint32_t& latea, uint32_t& lateb) {
+                              latea = nexta + ga * opaque_zero;
+                              lateb = nextb + gb * opaque_zero;
+                          },
+                          args);
 }
 
 template <int kRegs>
@@ -850,6 +869,154 @@ __global__ void __maxnreg__(kRegs) ScanUniformLook2Kernel(const __grid_constant_
                     if (!more_a || __all_sync(0xffffffffu, (sv.noexit[ga] & sv.noexit[gb]) != 0))
                         break;
                 }
+            }
+        }
+        const uint64_t ia = (uint64_t) pair * 64 + (threadIdx.x & 31);
+        LaneState s;
+        s.g = t.H;
+        s.cold = ga == t.H ? preva : ga;
+        Report(a, t, s, 2 * (uint64_t) pair, ia, ia < a.n);
+        if (second) {
+            s.cold = gb == t.H ? prevb : gb;
+            Report(a, t, s, 2 * (uint64_t) pair + 1, ia + 32, ia + 32 < a.n);
+        }
+    }
+}
+
+// ---------------------------------------------------------------- LOOK variant, two strings per lane, fed from a ring
+//
+// ScanUniformLook2Kernel keeps one 32-byte block of each string in flight, and that load shape alone moves about half of
+// what HBM can deliver: the scan is bound by its loads, not by the walk.  More blocks in flight per string would take
+// registers the kernel does not have, so here each lane copies its blocks with cp.async (LDGSTS) into a private ring in
+// shared memory, three slots per string, and reads a block into registers (two LDS.128 per string) only when it walks
+// it: two blocks of each string are on their way while one is walked.  Same walk, same pairs of units, same NoExit exit
+// every 64 bytes; one CTA of 24 warps per SM.  The shape is the fastest of the ring shapes tools/microbench.cu measures
+// without the walk (DESIGN.md section 4): 24 warps x 3 slots beat 28 x 2 and 32 x 2.
+// A slot of a warp is two 512-byte rows, one per 16-byte half, so the copies and the reads of a warp are free of bank
+// conflicts: per warp, slot k of string s (0, 1) sits at k * 2048 + s * 1024, its second half 512 bytes further.
+constexpr int kRingBlock = 768;
+constexpr uint32_t kRingSlots = 3;
+constexpr uint32_t kRingSlotBytes = 2048;
+constexpr size_t kRingWarpBytes = (size_t) kRingSlots * kRingSlotBytes;      // 6 KB; 144 KB per CTA beside <= 75.5 KB of tables
+
+__device__ __forceinline__ uint32_t NextSlot(uint32_t slot) { return slot + kRingSlotBytes == kRingWarpBytes ? 0 : slot + kRingSlotBytes; }
+
+// One 32-byte block of a string into its slot.  cp.async.cg: both 16-byte halves go to L2, which in the ring measured
+// faster than .ca (the register loads are the other way round); the first half carries the 128-byte L2 prefetch-size
+// hint of LoadStream32, so that an L2 miss fetches the line that holds the string's next three blocks.
+__device__ __forceinline__ void CopyBlock32(uint32_t dst_shared, const uint8_t* src)
+{
+    asm volatile("cp.async.cg.shared.global.L2::128B [%0], [%1], 16;\n\t"
+                 "cp.async.cg.shared.global [%2], [%3], 16;" ::"r"(dst_shared), "l"(src), "r"(dst_shared + 512), "l"(src + 16)
+                 : "memory");
+}
+
+__device__ __forceinline__ uint32_t LoadShared4(uint32_t shared_addr)
+{
+    uint32_t v;
+    asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(shared_addr) : "memory");
+    return v;
+}
+
+// The first words of the next blocks, read after the walk of this block's first 28 bytes once their commit group has
+// landed.  The address depends on the walk (plus g times a kernel argument that is always zero), so the read cannot be
+// hoisted to where the copy may still be in flight.
+struct RingNext {
+    uint32_t at;          // the next block's slot, string a; string b 1024 bytes further
+    uint32_t zero;
+    __device__ __forceinline__ void operator()(uint32_t ga, uint32_t gb, uint32_t& latea, uint32_t& lateb) const
+    {
+        CopyAsyncWait<kRingSlots - 1>();
+        latea = LoadShared4(at + ga * zero);
+        lateb = LoadShared4(at + 1024 + gb * zero);
+    }
+};
+
+__global__ void __launch_bounds__(kRingBlock, 1) ScanUniformLookRingKernel(const __grid_constant__ ScanArgs a)
+{
+    uint8_t* const smem = pire_b200_smem;
+    SharedView sv = CarveShared(smem, a.hot);
+    StageTables(a, sv, a.hot8, a.hot);
+
+    Tables t;
+    t.hot = sv.hot;
+    t.base = SmemWindowBase();
+    t.cls = sv.cls;
+    t.full = a.full;
+    t.H = a.hot;
+    t.letters = a.letters;
+    t.wide = a.wide;
+    t.m0 = a.look_bitmap;
+    LookFilter f;
+    f.lo = a.look_bitmap;
+    f.hi = 0;
+    f.zero = a.opaque_zero;
+    f.rev = __brev(f.lo);
+
+    const uint32_t units = (uint32_t) ((a.n + 31) / 32);
+    const uint32_t pairs = (units + 1) / 2;
+    const uint32_t warps_per_block = blockDim.x >> 5;
+    const uint32_t warps = gridDim.x * warps_per_block;
+    const uint32_t len = (uint32_t) a.fixed_len;
+    const uint32_t blocks = len >> 5;
+    // this lane's 16-byte column of its warp's ring (slot 0, string a, first half)
+    const uint32_t ring = SmemAddr(sv.stage) + (threadIdx.x >> 5) * (uint32_t) kRingWarpBytes + (threadIdx.x & 31) * 16;
+
+    for (uint32_t pair = blockIdx.x * warps_per_block + (threadIdx.x >> 5); pair < pairs; pair += warps) {
+        const bool second = 2 * pair + 1 < units;          // the last pair of an odd batch walks its first unit twice
+        uint32_t ga, preva, gb, prevb;
+        {
+            const uint64_t ia = (uint64_t) pair * 64 + (threadIdx.x & 31);
+            const uint64_t ib = ia + (second ? 32 : 0);
+            const uint8_t* pa = a.corpus + (ia < a.n ? ia : a.n - 1) * (uint64_t) len;
+            const uint8_t* pb = a.corpus + (ib < a.n ? ib : a.n - 1) * (uint64_t) len;
+            preva = prevb = a.start;
+            ga = gb = a.start < t.H ? a.start : t.H;
+            if (blocks != 0) {
+                // Blocks 0..2 of both strings, one commit group per block (empty past the end); block k + 3 refills the
+                // slot of block k as soon as block k is in registers.  No copy reaches past the end of a string: the
+                // last string of a batch may end where its allocation ends.
+#pragma unroll
+                for (uint32_t j = 0; j < kRingSlots; ++j) {
+                    if (j < blocks) {
+                        CopyBlock32(ring + j * kRingSlotBytes, pa + 32 * j);
+                        CopyBlock32(ring + j * kRingSlotBytes + 1024, pb + 32 * j);
+                    }
+                    CopyAsyncCommit();
+                }
+                CopyAsyncWait<kRingSlots - 1>();                    // block 0 has landed
+                uint32_t s0 = 0;                                    // slot of block k
+                for (uint32_t k = 0;; k += 2) {
+                    // block k (landed: the prologue's wait or the previous block's late one)
+                    const uint32_t s1 = NextSlot(s0);
+                    uint4 a0 = LoadShared16(ring + s0), a1 = LoadShared16(ring + s0 + 512);
+                    uint4 b0 = LoadShared16(ring + s0 + 1024), b1 = LoadShared16(ring + s0 + 1536);
+                    if (k + kRingSlots < blocks) {
+                        CopyBlock32(ring + s0, pa + 32 * (size_t) (k + kRingSlots));
+                        CopyBlock32(ring + s0 + 1024, pb + 32 * (size_t) (k + kRingSlots));
+                    }
+                    CopyAsyncCommit();
+                    const bool more_1 = k + 1 < blocks;
+                    LookBlock32x2<true>(t, ga, preva, a0, a1, gb, prevb, b0, b1, more_1, f, RingNext{ring + s1, a.opaque_zero}, &a);
+                    if (!more_1)
+                        break;
+                    // block k + 1
+                    const uint32_t s2 = NextSlot(s1);
+                    a0 = LoadShared16(ring + s1), a1 = LoadShared16(ring + s1 + 512);
+                    b0 = LoadShared16(ring + s1 + 1024), b1 = LoadShared16(ring + s1 + 1536);
+                    if (k + 1 + kRingSlots < blocks) {
+                        CopyBlock32(ring + s1, pa + 32 * (size_t) (k + 1 + kRingSlots));
+                        CopyBlock32(ring + s1 + 1024, pb + 32 * (size_t) (k + 1 + kRingSlots));
+                    }
+                    CopyAsyncCommit();
+                    const bool more_2 = k + 2 < blocks;
+                    LookBlock32x2<true>(t, ga, preva, a0, a1, gb, prevb, b0, b1, more_2, f, RingNext{ring + s2, a.opaque_zero}, &a);
+                    // multi.h:955-958,:979-982 (NoExit), looked at every 64 bytes
+                    if (!more_2 || __all_sync(0xffffffffu, (sv.noexit[ga] & sv.noexit[gb]) != 0))
+                        break;
+                    s0 = s2;
+                }
+                CopyAsyncWait<0>();            // a NoExit exit leaves copies in flight: they land before the slots are reused
             }
         }
         const uint64_t ia = (uint64_t) pair * 64 + (threadIdx.x & 31);
@@ -2991,10 +3158,24 @@ int LookIlpRegs()
     return regs;
 }
 
+// The two-string look-ahead kernel is fed from the cp.async ring (ScanUniformLookRingKernel) unless PIRE_B200_LOOK_RING=0,
+// which selects the register-fed ScanUniformLook2Kernel; so does an explicit PIRE_B200_LOOK_ILP_REGS, which names one of its
+// register budgets.
+bool LookRing()
+{
+    static const bool ring = [] {
+        const char* env = getenv("PIRE_B200_LOOK_RING");
+        return !(env && atoi(env) == 0) && !getenv("PIRE_B200_LOOK_ILP_REGS");
+    }();
+    return ring;
+}
+
 const void* KernelFor(int variant, bool uniform)
 {
     if (variant == kVariantPriv && uniform)
         return reinterpret_cast<const void*>(&ScanUniformPrivKernel);
+    if (variant == kVariantLook && uniform && LookIlp() == 2 && LookRing())
+        return reinterpret_cast<const void*>(&ScanUniformLookRingKernel);
     if (variant == kVariantLook && uniform && LookIlp() == 2)
         return LookIlpRegs() == 64   ? reinterpret_cast<const void*>(&ScanUniformLook2Kernel<64>)
                : LookIlpRegs() == 80 ? reinterpret_cast<const void*>(&ScanUniformLook2Kernel<80>)
@@ -3055,11 +3236,13 @@ cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv
             return env && atoi(env) >= 32 && atoi(env) <= 1024 && atoi(env) % 32 == 0 ? atoi(env) : 0;
         }();
         if (variant == kVariantLook && LookIlp() == 2)
-            plan->block = LookIlpRegs() == 64 ? 512 : LookIlpRegs() == 80 ? 384 : 448;
+            plan->block = LookRing() ? kRingBlock : LookIlpRegs() == 64 ? 512 : LookIlpRegs() == 80 ? 384 : 448;
         if (look_block)
             plan->block = look_block;
     }
     plan->shared = priv ? ScanSharedBytes(hot_small, priv_rows) : uniform ? ScanSharedBytes(hot, 0) : GenericSharedBytes(hot);
+    if (variant == kVariantLook && uniform && LookIlp() == 2 && LookRing())
+        plan->shared += (size_t) (plan->block / 32) * kRingWarpBytes;         // every warp's ring after the tables
     int sms = 0, per_sm = 0;
     cudaError_t err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     if (err != cudaSuccess)
@@ -3081,7 +3264,7 @@ cudaError_t LaunchScan(const ScanArgs& a, int variant, bool uniform, const Launc
         return cudaSuccess;
     uint64_t units = (a.n + 31) / 32;
     if (variant == kVariantLook && uniform && LookIlp() == 2)
-        units = (units + 1) / 2;              // a warp of ScanUniformLook2Kernel takes two units at a time
+        units = (units + 1) / 2;              // a warp of ScanUniformLook2Kernel / ScanUniformLookRingKernel takes two units at a time
     const uint64_t warps_per_block = (uint64_t) plan.block / 32;
     uint64_t want = (units + warps_per_block - 1) / warps_per_block;
     int grid = (int) (want < (uint64_t) plan.grid ? want : (uint64_t) plan.grid);

@@ -8,7 +8,9 @@
 // The "flagship" rows run at the glued scan's shapes: the register kernel's residency (two CTAs of 448 threads, 28
 // warps per SM) with two strings per lane (units 2p and 2p+1 of a pair, one 32-byte block of each in flight), and a
 // TMA-staged alternative (one CTA of 1024 threads per SM, a per-warp ring of 64-row x 32-byte tiles read with
-// LDS.128), the shape a shared-memory-fed walk would need beside a 75 KB hot table.
+// LDS.128), the shape a shared-memory-fed walk would need beside a 75 KB hot table.  The "ring" rows feed the same two
+// strings per lane from a per-lane cp.async ring in shared memory (one CTA per SM beside 76 KB held back for the table),
+// the input side of ScanUniformLookRingKernel, at several (warps, slots) shapes, .ca / .cg and L2 prefetch-size hints.
 //
 //   microbench [GiB=4] [string_len=1024]
 #include <cuda.h>
@@ -168,6 +170,82 @@ __global__ void __launch_bounds__(1024, 1) TmaTileKernel(const __grid_constant__
             IssueTile(ring + slot * kTileBytes, bars + 8 * slot, &tm, (next % chunks) * 32, (first + next / chunks * warps) * 64);
         }
     }
+    if (acc == 0x12345678u)
+        out[0] = acc;
+}
+
+// ---- per-lane cp.async ring: the input side of a two-string kernel that keeps kSlots 32-byte blocks of each string in
+// shared memory (LDGSTS), read back with LDS.128.  One CTA per SM beside 76 KB held back for the hot table.  A slot of a
+// warp is two 512-byte rows, one per 16-byte half, so that the copies and the reads of a warp are free of bank conflicts.
+constexpr uint32_t kRingTableBytes = 76 * 1024;
+
+// One 32-byte block into a slot: kCg = cp.async.cg (both halves to L2, L1 bypassed) or .ca (allocating in L1, so the
+// second half is an L1 hit); the first half carries the kL2-byte prefetch-size hint.
+template <bool kCg, int kL2>
+__device__ __forceinline__ void CopyBlock(uint32_t dst, const uint8_t* src)
+{
+#define RING_COPY(LEVEL, HINT)                                                                                       \
+    asm volatile("cp.async." LEVEL ".shared.global" HINT " [%0], [%1], 16;\n\t"                                     \
+                 "cp.async." LEVEL ".shared.global [%2], [%3], 16;" ::"r"(dst), "l"(src), "r"(dst + 512), "l"(src + 16) \
+                 : "memory")
+    if (kCg && kL2 == 64)
+        RING_COPY("cg", ".L2::64B");
+    else if (kCg && kL2 == 128)
+        RING_COPY("cg", ".L2::128B");
+    else if (kCg)
+        RING_COPY("cg", ".L2::256B");
+    else if (kL2 == 64)
+        RING_COPY("ca", ".L2::64B");
+    else if (kL2 == 128)
+        RING_COPY("ca", ".L2::128B");
+    else
+        RING_COPY("ca", ".L2::256B");
+#undef RING_COPY
+}
+
+__device__ __forceinline__ uint4 Lds16(uint32_t at)
+{
+    uint4 v;
+    asm volatile("ld.shared.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(at) : "memory");
+    return v;
+}
+
+template <bool kCg, int kL2, int kSlots>
+__global__ void __launch_bounds__(1024, 1) LoadRingKernel(const uint8_t* corpus, uint64_t n, uint32_t len, uint32_t* out)
+{
+    extern __shared__ __align__(1024) uint8_t ring_smem[];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t warps = (uint64_t) gridDim.x * (blockDim.x / 32);
+    // slot k of string s (0, 1) of this lane: ring + (k * 2 + s) * 1024, second half 512 bytes further
+    const uint32_t ring = (uint32_t) __cvta_generic_to_shared(ring_smem) + kRingTableBytes + warp * kSlots * 2048 + lane * 16;
+    const uint32_t blocks = len / 32;
+    uint32_t acc = 0;
+    for (uint64_t pair = (uint64_t) blockIdx.x * (blockDim.x / 32) + warp; pair < n / 64; pair += warps) {
+        const uint8_t* pa = corpus + (pair * 64 + lane) * (uint64_t) len;
+        const uint8_t* pb = pa + 32 * (uint64_t) len;
+#pragma unroll
+        for (uint32_t k = 0; k < kSlots; ++k) {
+            if (k < blocks) {
+                CopyBlock<kCg, kL2>(ring + k * 2048, pa + 32 * k);
+                CopyBlock<kCg, kL2>(ring + k * 2048 + 1024, pb + 32 * k);
+            }
+            asm volatile("cp.async.commit_group;" ::: "memory");
+        }
+        uint32_t slot = 0;
+        for (uint32_t k = 0; k < blocks; ++k) {
+            asm volatile("cp.async.wait_group %0;" ::"n"(kSlots - 1) : "memory");
+            const uint32_t at = ring + slot * 2048;
+            const uint4 a0 = Lds16(at), a1 = Lds16(at + 512), b0 = Lds16(at + 1024), b1 = Lds16(at + 1536);
+            if (k + kSlots < blocks) {
+                CopyBlock<kCg, kL2>(at, pa + 32 * (k + kSlots));
+                CopyBlock<kCg, kL2>(at + 1024, pb + 32 * (k + kSlots));
+            }
+            asm volatile("cp.async.commit_group;" ::: "memory");
+            acc ^= Fold(a0) ^ Fold(a1) ^ Fold(b0) ^ Fold(b1);
+            slot = slot + 1 == kSlots ? 0 : slot + 1;
+        }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
     if (acc == 0x12345678u)
         out[0] = acc;
 }
@@ -360,6 +438,26 @@ void RunTma(const char* name, const uint8_t* d, uint64_t n, uint32_t len, uint32
     Report(name, 1024, n, len, Best([&] { TmaTileKernel<kStages><<<sms, 1024, smem>>>(tm, n, len, out); }));
 }
 
+template <bool kCg, int kL2, int kSlots>
+void RunRing(const uint8_t* d, uint64_t n, uint32_t len, uint32_t* out, int warps)
+{
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+    const size_t smem = kRingTableBytes + (size_t) warps * kSlots * 2048;
+    CK(cudaFuncSetAttribute(LoadRingKernel<kCg, kL2, kSlots>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+    char name[96];
+    std::snprintf(name, sizeof name, "ring_cp_async_%s_l2_%dB_%dwarps_%dslots", kCg ? "cg" : "ca", kL2, warps, kSlots);
+    Report(name, warps * 32, n, len, Best([&] { LoadRingKernel<kCg, kL2, kSlots><<<sms, warps * 32, smem>>>(d, n, len, out); }));
+}
+
+template <bool kCg, int kL2>
+void RunRingShapes(const uint8_t* d, uint64_t n, uint32_t len, uint32_t* out)
+{
+    RunRing<kCg, kL2, 2>(d, n, len, out, 32);
+    RunRing<kCg, kL2, 2>(d, n, len, out, 28);
+    RunRing<kCg, kL2, 3>(d, n, len, out, 24);
+}
+
 int main(int argc, char** argv)
 {
     const double gib = argc > 1 ? std::atof(argv[1]) : 4.0;
@@ -386,6 +484,13 @@ int main(int argc, char** argv)
         Report("two_strings_l2_256B", 896, n, len, Best([&] { LoadPairKernel<256><<<sms * 2, 448>>>(d, n, len, out); }));
         RunTma<2>("flagship_tma_tile_64x32_swz32_2stages", d, n, len, out);
         RunTma<3>("tma_tile_64x32_swz32_3stages", d, n, len, out);
+        // two strings per lane fed from a per-lane cp.async ring, at (warps, slots) = (32, 2), (28, 2), (24, 3)
+        RunRingShapes<false, 64>(d, n, len, out);
+        RunRingShapes<false, 128>(d, n, len, out);
+        RunRingShapes<false, 256>(d, n, len, out);
+        RunRingShapes<true, 64>(d, n, len, out);
+        RunRingShapes<true, 128>(d, n, len, out);
+        RunRingShapes<true, 256>(d, n, len, out);
     }
     for (int tps : {1024, 1536, 2048}) {
         Run<5>("coalesced_ldg128", d, n, len, out, tps);
