@@ -63,7 +63,10 @@ enum {
     PIRE_GPU_VARIANT_LOOK1 = 6,    /* LOOK walks two strings per lane on fixed-length batches (the second string's step fills
                                       the latency of the first one's table read); LOOK1 is the same filter with one string per
                                       lane -- the shape for batches too small to give every resident warp two units */
-    PIRE_GPU_VARIANT_SLOTS = 8     /* length of per-variant arrays indexed by variant id */
+    PIRE_GPU_VARIANT_LOOK_RING1 = 7, /* LOOK1's walk, one string per lane, fed from a ring in shared memory that keeps two
+                                      more 32-byte blocks of every string in flight (fixed-length batches; the CSR
+                                      look-ahead kernel otherwise) */
+    PIRE_GPU_VARIANT_SLOTS = 8    /* length of per-variant arrays indexed by variant id */
 };
 
 typedef struct pire_gpu_info {

@@ -20,9 +20,10 @@ RUN_BEGIN = 1
 RUN_END = 2
 RUN_LINES = 4
 VARIANT_AUTO, VARIANT_PLAIN, VARIANT_PRED, VARIANT_PRIV, VARIANT_LOOK, VARIANT_LOOK64, VARIANT_LOOK1 = 0, 1, 2, 3, 4, 5, 6
+VARIANT_LOOK_RING1 = 7
 VARIANT_SLOTS = 8
 VARIANT_NAMES = {VARIANT_PLAIN: "plain", VARIANT_PRED: "pred", VARIANT_PRIV: "priv", VARIANT_LOOK: "look", VARIANT_LOOK64: "look64",
-                 VARIANT_LOOK1: "look1"}
+                 VARIANT_LOOK1: "look1", VARIANT_LOOK_RING1: "look_ring1"}
 
 # every symbol include/pire_b200.h declares
 SYMBOLS = [

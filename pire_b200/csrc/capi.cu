@@ -55,7 +55,7 @@ void DeviceTables::Free()
 
 uint32_t ResolveVariant(const pire_gpu_scanner* sc, bool uniform)
 {
-    if (sc->variant >= PIRE_GPU_VARIANT_PLAIN && sc->variant <= PIRE_GPU_VARIANT_LOOK1) {
+    if (sc->variant >= PIRE_GPU_VARIANT_PLAIN && sc->variant <= PIRE_GPU_VARIANT_LOOK_RING1) {
         if (sc->variant >= PIRE_GPU_VARIANT_LOOK && !sc->tab.look_ok)
             return PIRE_GPU_VARIANT_PRED;       // an exit of the resting state is cold: no look-ahead set
         return sc->variant;
@@ -135,7 +135,7 @@ int Upload(pire_gpu_scanner* sc)
     if (!t.new_of_old.empty())
         CUDA_TRY(cudaMemcpy(d.new_of_old, t.new_of_old.data(), t.new_of_old.size() * 4, cudaMemcpyHostToDevice));
     sc->priv_ok = false;
-    for (int v = kVariantPlain; v <= kVariantLook1; ++v)
+    for (int v = kVariantPlain; v <= kVariantLookRing1; ++v)
         for (int u = 0; u < 2; ++u) {
             cudaError_t pe = PlanScan(sc->device, t.hot, t.hot_small, t.priv_rows, v, u != 0, &sc->plan[v][u]);
             if (v == kVariantPriv && u == 1) {
@@ -288,7 +288,7 @@ int pire_gpu_scanner_info(const pire_gpu_scanner* sc, pire_gpu_info* out)
 
 int pire_gpu_scanner_set_variant(pire_gpu_scanner* sc, uint32_t variant)
 {
-    if (!sc || variant > PIRE_GPU_VARIANT_LOOK1)
+    if (!sc || variant > PIRE_GPU_VARIANT_LOOK_RING1)
         return Fail(PIRE_GPU_EINVAL, "bad variant");
     sc->variant = variant;
     return PIRE_GPU_OK;
@@ -689,12 +689,12 @@ int pire_gpu_scanner_autoselect(pire_gpu_scanner* sc, const uint8_t* d_corpus, c
     const uint32_t saved = sc->variant;
     uint32_t best = 0;
     float best_ms = 0.f;
-    for (uint32_t v = PIRE_GPU_VARIANT_PLAIN; v <= PIRE_GPU_VARIANT_LOOK1 && ce == cudaSuccess; ++v) {
+    for (uint32_t v = PIRE_GPU_VARIANT_PLAIN; v <= PIRE_GPU_VARIANT_LOOK_RING1 && ce == cudaSuccess; ++v) {
         if (v == PIRE_GPU_VARIANT_PRIV && !(uniform && sc->priv_ok))
             continue;
         if (v >= PIRE_GPU_VARIANT_LOOK && !sc->tab.look_ok)
             continue;
-        if ((v == PIRE_GPU_VARIANT_LOOK64 || v == PIRE_GPU_VARIANT_LOOK1) && !uniform)
+        if ((v == PIRE_GPU_VARIANT_LOOK64 || v == PIRE_GPU_VARIANT_LOOK1 || v == PIRE_GPU_VARIANT_LOOK_RING1) && !uniform)
             continue;               // CSR batches have one look-ahead kernel
         sc->variant = v;
         float ms = 0.f;

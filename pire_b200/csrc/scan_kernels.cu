@@ -22,7 +22,8 @@
 //   * LOOK variant (the glued benchmark scan): the filter looks one byte further -- a resting
 //     lane reads the table only if this byte and the next both pass -- in 5.5 instructions per
 //     byte (LookProbe / LookStep), two strings per lane (ScanUniformLookRingKernel, fed from a per-lane cp.async ring
-//     with two blocks of each string in flight; ScanUniformLook2Kernel, fed from registers).
+//     with two blocks of each string in flight; ScanUniformLook2Kernel, fed from registers).  The LOOK_RING1 variant walks
+//     one string per lane from such a ring, 32 warps per SM (ScanUniformLookRing1Kernel).
 //   * Input bytes: each lane streams its own string: 32-byte read-only loads (two
 //     LDG.128 of one sector, the second an L1 hit), one ahead in a register ping-pong (uniform kernels,
 //     two LDG.128 per 32 bytes), or a four-deep cp.async ring of 16-byte chunks in shared memory
@@ -594,9 +595,11 @@ __device__ __noinline__ uint32_t ReplayBlock32(const ScanArgs* a, uint32_t from,
     return ReplayChunk(sv.hot, sv.cls, a->full, a->hot, letters_wide, mid, v1);
 }
 
-template <bool k64, bool kClean = false>
+// `late(g)` fetches the first word of the block that follows, after the walk of the block's first 28 bytes: from registers
+// loaded a block ahead (ScanUniformLookKernel) or from the ring in shared memory (ScanUniformLookRing1Kernel).
+template <bool k64, bool kClean, typename Late>
 __device__ __forceinline__ void LookBlock32(const Tables& t, uint32_t& g, uint32_t& prev, const uint4& v0, const uint4& v1,
-                                            uint32_t next0, bool more, const LookFilter& f, uint32_t opaque_zero, const ScanArgs* args)
+                                            bool more, const LookFilter& f, Late late, const ScanArgs* args)
 {
     prev = g == t.H ? prev : g;
     uint32_t bb, pa, bn, pn;
@@ -615,18 +618,23 @@ __device__ __forceinline__ void LookBlock32(const Tables& t, uint32_t& g, uint32
     LookWord<k64, kClean>(g, v1.y, bn, pn, pa, t.base, f);
     LookProbe<k64, 0, kClean>(v1.w, t.base, f, bn, pn);
     LookWord<k64, kClean>(g, v1.z, bb, pa, pn, t.base, f);
-    // The word after the block was requested from HBM when this block began: its probe must stay down here (an
-    // ordinary intrinsic is hoisted to the top of the block by the compiler, where it waits for the whole DRAM
-    // latency).
-    // (a volatile mov is not enough: ptxas schedules across it.  The word is made to depend on the walk itself --
-    // plus g times a kernel argument that is always zero -- which costs one IMAD per block.)
-    const uint32_t late = next0 + g * opaque_zero;
-    LookProbe<k64, 0, kClean>(late, t.base, f, bb, pa);
+    LookProbe<k64, 0, kClean>(late(g), t.base, f, bb, pa);
     LookWord<k64, kClean>(g, v1.w, bn, pn, more ? pa : (kClean ? 0x80000000u : 0xffffffffu), t.base, f);
     if (g == t.H) {
         prev = ReplayBlock32(args, prev, v0, v1);
         g = prev < t.H ? prev : t.H;
     }
+}
+
+// The word after the block was requested from HBM when this block began: its probe must stay down here (an ordinary
+// intrinsic is hoisted to the top of the block by the compiler, where it waits for the whole DRAM latency).
+// (a volatile mov is not enough: ptxas schedules across it.  The word is made to depend on the walk itself -- plus g
+// times a kernel argument that is always zero -- which costs one IMAD per block.)
+template <bool k64, bool kClean = false>
+__device__ __forceinline__ void LookBlock32(const Tables& t, uint32_t& g, uint32_t& prev, const uint4& v0, const uint4& v1,
+                                            uint32_t next0, bool more, const LookFilter& f, uint32_t opaque_zero, const ScanArgs* args)
+{
+    LookBlock32<k64, kClean>(t, g, prev, v0, v1, more, f, [=](uint32_t g) { return next0 + g * opaque_zero; }, args);
 }
 
 // Register budget.  The register file is split between the four warp schedulers (16 K registers each), so a
@@ -1028,6 +1036,120 @@ __global__ void __launch_bounds__(kRingBlock, 1) ScanUniformLookRingKernel(const
             s.cold = gb == t.H ? prevb : gb;
             Report(a, t, s, 2 * (uint64_t) pair + 1, ia + 32, ia + 32 < a.n);
         }
+    }
+}
+
+// ---------------------------------------------------------------- LOOK variant, one string per lane, fed from a ring
+//
+// Two strings per lane were made for the register-fed kernel, which was short of independent chains and of registers.
+// With the input in a ring the registers are free again: a one-string walk needs one block's eight data registers and
+// the late word, so 32 warps fit in one CTA.  Here each lane walks one string (ScanUniformLookKernel's walk: 32-slot
+// filter, clean probes) from a ring of kSlots blocks; kSlots - 1 blocks of every string are on their way while one is
+// walked, and half as many lines are in progress in L2 as with two strings per lane.  NoExit exit every 64 bytes, as in
+// the other look-ahead kernels.  The shape, one CTA of 32 warps per SM with three slots (96 KB of ring), is the fastest
+// of the walk at 16 x 8, 24 x 6, 28 x 5, 32 x 3 and 32 x 4 (DESIGN.md section 4): fewer warps starve the walk of
+// chains even where their loads alone run faster.  A slot of a warp is two 512-byte rows, one per 16-byte half, so the
+// copies and the reads of a warp are free of bank conflicts: per warp, slot k sits at k * 1024.
+constexpr int kRing1Block = 1024;
+constexpr int kRing1Slots = 3;
+constexpr uint32_t kRing1SlotBytes = 1024;
+template <int kSlots>
+__device__ __forceinline__ uint32_t NextSlot1(uint32_t slot) { return slot + kRing1SlotBytes == kSlots * kRing1SlotBytes ? 0 : slot + kRing1SlotBytes; }
+
+// The first word of the next block, read after the walk of this block's first 28 bytes once its commit group has landed;
+// the address depends on the walk, as in RingNext.
+template <int kSlots>
+struct RingNext1 {
+    uint32_t at;          // the next block's slot
+    uint32_t zero;
+    __device__ __forceinline__ uint32_t operator()(uint32_t g) const
+    {
+        CopyAsyncWait<kSlots - 1>();
+        return LoadShared4(at + g * zero);
+    }
+};
+
+template <int kSlots>
+__global__ void __launch_bounds__(kRing1Block, 1) ScanUniformLookRing1Kernel(const __grid_constant__ ScanArgs a)
+{
+    uint8_t* const smem = pire_b200_smem;
+    SharedView sv = CarveShared(smem, a.hot);
+    StageTables(a, sv, a.hot8, a.hot);
+
+    Tables t;
+    t.hot = sv.hot;
+    t.base = SmemWindowBase();
+    t.cls = sv.cls;
+    t.full = a.full;
+    t.H = a.hot;
+    t.letters = a.letters;
+    t.wide = a.wide;
+    t.m0 = a.look_bitmap;
+    LookFilter f;
+    f.lo = a.look_bitmap;
+    f.hi = 0;
+    f.zero = a.opaque_zero;
+    f.rev = __brev(f.lo);
+
+    const uint32_t units = (uint32_t) ((a.n + 31) / 32);
+    const uint32_t warps_per_block = blockDim.x >> 5;
+    const uint32_t warps = gridDim.x * warps_per_block;
+    const uint32_t len = (uint32_t) a.fixed_len;
+    const uint32_t blocks = len >> 5;
+    // this lane's 16-byte column of its warp's ring (slot 0, first half)
+    const uint32_t ring = SmemAddr(sv.stage) + (threadIdx.x >> 5) * (uint32_t) (kSlots * kRing1SlotBytes) + (threadIdx.x & 31) * 16;
+
+    for (uint32_t unit = blockIdx.x * warps_per_block + (threadIdx.x >> 5); unit < units; unit += warps) {
+        uint32_t g, prev;
+        {
+            const uint64_t i = (uint64_t) unit * 32 + (threadIdx.x & 31);
+            const uint8_t* p = a.corpus + (i < a.n ? i : a.n - 1) * (uint64_t) len;
+            prev = a.start;
+            g = a.start < t.H ? a.start : t.H;
+            if (blocks != 0) {
+                // Blocks 0..kSlots-1, one commit group per block (empty past the end); block k + kSlots refills the slot
+                // of block k as soon as block k is in registers.  No copy reaches past the end of a string: the last
+                // string of a batch may end where its allocation ends.
+#pragma unroll
+                for (uint32_t j = 0; j < kSlots; ++j) {
+                    if (j < blocks)
+                        CopyBlock32(ring + j * kRing1SlotBytes, p + 32 * j);
+                    CopyAsyncCommit();
+                }
+                CopyAsyncWait<kSlots - 1>();                        // block 0 has landed
+                uint32_t s0 = 0;                                    // slot of block k
+                for (uint32_t k = 0;; k += 2) {
+                    // block k (landed: the prologue's wait or the previous block's late one)
+                    const uint32_t s1 = NextSlot1<kSlots>(s0);
+                    uint4 v0 = LoadShared16(ring + s0), v1 = LoadShared16(ring + s0 + 512);
+                    if (k + kSlots < blocks)
+                        CopyBlock32(ring + s0, p + 32 * (size_t) (k + kSlots));
+                    CopyAsyncCommit();
+                    const bool more_1 = k + 1 < blocks;
+                    LookBlock32<false, true>(t, g, prev, v0, v1, more_1, f, RingNext1<kSlots>{ring + s1, a.opaque_zero}, &a);
+                    if (!more_1)
+                        break;
+                    // block k + 1
+                    const uint32_t s2 = NextSlot1<kSlots>(s1);
+                    v0 = LoadShared16(ring + s1), v1 = LoadShared16(ring + s1 + 512);
+                    if (k + 1 + kSlots < blocks)
+                        CopyBlock32(ring + s1, p + 32 * (size_t) (k + 1 + kSlots));
+                    CopyAsyncCommit();
+                    const bool more_2 = k + 2 < blocks;
+                    LookBlock32<false, true>(t, g, prev, v0, v1, more_2, f, RingNext1<kSlots>{ring + s2, a.opaque_zero}, &a);
+                    // multi.h:955-958,:979-982 (NoExit), looked at every 64 bytes
+                    if (!more_2 || __all_sync(0xffffffffu, sv.noexit[g] != 0))
+                        break;
+                    s0 = s2;
+                }
+                CopyAsyncWait<0>();            // a NoExit exit leaves copies in flight: they land before the slots are reused
+            }
+        }
+        const uint64_t i = (uint64_t) unit * 32 + (threadIdx.x & 31);
+        LaneState s;
+        s.g = t.H;
+        s.cold = g == t.H ? prev : g;
+        Report(a, t, s, unit, i, i < a.n);
     }
 }
 
@@ -3170,10 +3292,14 @@ bool LookRing()
     return ring;
 }
 
+// The one-string ring kernel keeps 8 slots per string in 16 warps; PIRE_B200_LOOK_RING1_SLOTS=6 selects 6 slots in 24
+// warps, the same 144 KB of ring per SM as the two-string kernel (experiments).
 const void* KernelFor(int variant, bool uniform)
 {
     if (variant == kVariantPriv && uniform)
         return reinterpret_cast<const void*>(&ScanUniformPrivKernel);
+    if (variant == kVariantLookRing1 && uniform)
+        return reinterpret_cast<const void*>(&ScanUniformLookRing1Kernel<kRing1Slots>);
     if (variant == kVariantLook && uniform && LookIlp() == 2 && LookRing())
         return reinterpret_cast<const void*>(&ScanUniformLookRingKernel);
     if (variant == kVariantLook && uniform && LookIlp() == 2)
@@ -3191,8 +3317,8 @@ const void* KernelFor(int variant, bool uniform)
                                 : reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 40>);
     if (uniform)
         return variant == kVariantPred ? UniformKernelPtr<true>() : UniformKernelPtr<false>();
-    if (variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1)      // CSR batches: one look-ahead kernel (32-slot filter)
-        return GenericKernelPtr<2>();
+    if (variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1 || variant == kVariantLookRing1)
+        return GenericKernelPtr<2>();         // CSR batches: one look-ahead kernel (32-slot filter)
     return variant == kVariantPred ? GenericKernelPtr<1>() : GenericKernelPtr<0>();
 }
 
@@ -3210,7 +3336,8 @@ cudaError_t PrepareScanKernels(int device)
     err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
     if (err != cudaSuccess)
         return err;
-    for (int variant : {(int) kVariantPlain, (int) kVariantPred, (int) kVariantPriv, (int) kVariantLook, (int) kVariantLook64, (int) kVariantLook1})
+    for (int variant : {(int) kVariantPlain, (int) kVariantPred, (int) kVariantPriv, (int) kVariantLook, (int) kVariantLook64, (int) kVariantLook1,
+                        (int) kVariantLookRing1})
         for (bool uniform : {false, true}) {
             err = cudaFuncSetAttribute(KernelFor(variant, uniform), cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
             if (err != cudaSuccess)
@@ -3240,9 +3367,13 @@ cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv
         if (look_block)
             plan->block = look_block;
     }
+    if (variant == kVariantLookRing1 && uniform)
+        plan->block = kRing1Block;
     plan->shared = priv ? ScanSharedBytes(hot_small, priv_rows) : uniform ? ScanSharedBytes(hot, 0) : GenericSharedBytes(hot);
     if (variant == kVariantLook && uniform && LookIlp() == 2 && LookRing())
         plan->shared += (size_t) (plan->block / 32) * kRingWarpBytes;         // every warp's ring after the tables
+    if (variant == kVariantLookRing1 && uniform)
+        plan->shared += (size_t) (plan->block / 32) * kRing1Slots * kRing1SlotBytes;      // every warp's ring after the tables
     int sms = 0, per_sm = 0;
     cudaError_t err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     if (err != cudaSuccess)
@@ -3445,7 +3576,8 @@ cudaError_t LaunchLines(const ScanArgs& a, int variant, int device, cudaStream_t
     const bool in_stream = forced == 2 || (forced != 1 && a.start < a.hot);
     if (in_stream && !(a.start < a.hot))
         return cudaErrorInvalidValue;
-    const bool pred = variant == kVariantPred || variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1;
+    const bool pred = variant == kVariantPred || variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1
+                      || variant == kVariantLookRing1;
     const void* fn = in_stream ? (pred ? reinterpret_cast<const void*>(&ScanTextKernel<true>) : reinterpret_cast<const void*>(&ScanTextKernel<false>))
                                : (pred ? reinterpret_cast<const void*>(&ScanLinesKernel<true>) : reinterpret_cast<const void*>(&ScanLinesKernel<false>));
     const size_t shared = ScanSharedBytes(a.hot, 0) + (in_stream ? kTextFinBytes + kTextPackBytes : 0);

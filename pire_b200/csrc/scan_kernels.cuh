@@ -82,7 +82,15 @@ struct LaunchPlan {
     size_t shared = 0;
 };
 
-enum ScanVariant { kVariantPlain = 1, kVariantPred = 2, kVariantPriv = 3, kVariantLook = 4, kVariantLook64 = 5, kVariantLook1 = 6 };
+enum ScanVariant {
+    kVariantPlain = 1,
+    kVariantPred = 2,
+    kVariantPriv = 3,
+    kVariantLook = 4,
+    kVariantLook64 = 5,
+    kVariantLook1 = 6,
+    kVariantLookRing1 = 7
+};
 constexpr int kVariantSlots = 8;      // size of per-variant arrays (variant ids are 1-based)
 
 size_t ScanSharedBytes(uint32_t hot, uint32_t priv_rows);

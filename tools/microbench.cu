@@ -12,13 +12,17 @@
 // strings per lane from a per-lane cp.async ring in shared memory (one CTA per SM beside 76 KB held back for the table),
 // the input side of ScanUniformLookRingKernel, at several (warps, slots) shapes, .ca / .cg and L2 prefetch-size hints.
 //
-//   microbench [GiB=4] [string_len=1024]
+// The "ring1" rows keep one string per lane in the same kind of ring, the input side of ScanUniformLookRing1Kernel.
+//
+//   microbench [GiB=4] [string_len=1024] [ring]     ("ring": only the ring comparison rows; any other third argument:
+//                                                    only the pipe rows)
 #include <cuda.h>
 #include <cuda_runtime.h>
 
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
+#include <cstring>
 #include <vector>
 
 #define CK(x)                                                                                   \
@@ -250,6 +254,42 @@ __global__ void __launch_bounds__(1024, 1) LoadRingKernel(const uint8_t* corpus,
         out[0] = acc;
 }
 
+// The same ring with one string per lane (row 32u + lane of unit u): a warp's slot is 1 KB, two 512-byte rows (first and
+// second 16-byte halves of 32 lanes), so the same shared memory buys twice the depth per string.
+template <bool kCg, int kL2, int kSlots>
+__global__ void __launch_bounds__(1024, 1) LoadRing1Kernel(const uint8_t* corpus, uint64_t n, uint32_t len, uint32_t* out)
+{
+    extern __shared__ __align__(1024) uint8_t ring_smem[];
+    const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint64_t warps = (uint64_t) gridDim.x * (blockDim.x / 32);
+    const uint32_t ring = (uint32_t) __cvta_generic_to_shared(ring_smem) + kRingTableBytes + warp * kSlots * 1024 + lane * 16;
+    const uint32_t blocks = len / 32;
+    uint32_t acc = 0;
+    for (uint64_t unit = (uint64_t) blockIdx.x * (blockDim.x / 32) + warp; unit < n / 32; unit += warps) {
+        const uint8_t* p = corpus + (unit * 32 + lane) * (uint64_t) len;
+#pragma unroll
+        for (uint32_t k = 0; k < kSlots; ++k) {
+            if (k < blocks)
+                CopyBlock<kCg, kL2>(ring + k * 1024, p + 32 * k);
+            asm volatile("cp.async.commit_group;" ::: "memory");
+        }
+        uint32_t slot = 0;
+        for (uint32_t k = 0; k < blocks; ++k) {
+            asm volatile("cp.async.wait_group %0;" ::"n"(kSlots - 1) : "memory");
+            const uint32_t at = ring + slot * 1024;
+            const uint4 a0 = Lds16(at), a1 = Lds16(at + 512);
+            if (k + kSlots < blocks)
+                CopyBlock<kCg, kL2>(at, p + 32 * (k + kSlots));
+            asm volatile("cp.async.commit_group;" ::: "memory");
+            acc ^= Fold(a0) ^ Fold(a1);
+            slot = slot + 1 == kSlots ? 0 : slot + 1;
+        }
+    }
+    asm volatile("cp.async.wait_group 0;" ::: "memory");
+    if (acc == 0x12345678u)
+        out[0] = acc;
+}
+
 // mode 0: LDG.128 no_allocate, depth 1   mode 1: LDG.128 allocate (second half of the sector hits L1)
 // mode 2: 2 x LDG.128 per 32 B, no_allocate   mode 3: 2 x LDG.128 per 32 B, allocating in L1
 // mode 4: mode 3 with two 32-byte blocks in flight   mode 5: coalesced contiguous LDG.128 (upper bound)
@@ -458,6 +498,41 @@ void RunRingShapes(const uint8_t* d, uint64_t n, uint32_t len, uint32_t* out)
     RunRing<kCg, kL2, 3>(d, n, len, out, 24);
 }
 
+template <bool kCg, int kL2, int kSlots>
+void RunRing1(const uint8_t* d, uint64_t n, uint32_t len, uint32_t* out, int warps)
+{
+    int sms = 0;
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0));
+    const size_t smem = kRingTableBytes + (size_t) warps * kSlots * 1024;
+    CK(cudaFuncSetAttribute(LoadRing1Kernel<kCg, kL2, kSlots>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int) smem));
+    char name[96];
+    std::snprintf(name, sizeof name, "ring1_cp_async_%s_l2_%dB_%dwarps_%dslots", kCg ? "cg" : "ca", kL2, warps, kSlots);
+    Report(name, warps * 32, n, len, Best([&] { LoadRing1Kernel<kCg, kL2, kSlots><<<sms, warps * 32, smem>>>(d, n, len, out); }));
+}
+
+// One string per lane at (warps, slots) = (16, 8), (24, 4), (24, 6), (32, 3), (32, 4): 96 to 144 KB of ring.
+template <int kL2>
+void RunRing1Shapes(const uint8_t* d, uint64_t n, uint32_t len, uint32_t* out)
+{
+    RunRing1<true, kL2, 8>(d, n, len, out, 16);
+    RunRing1<true, kL2, 4>(d, n, len, out, 24);
+    RunRing1<true, kL2, 6>(d, n, len, out, 24);
+    RunRing1<true, kL2, 3>(d, n, len, out, 32);
+    RunRing1<true, kL2, 4>(d, n, len, out, 32);
+}
+
+// The shipped two-string ring next to the one-string shapes, and the two-string ring at 16 x 4 (the same 128 KB spent on
+// fewer strings), alternated twice so that drift between rows shows.
+void RunRingComparison(const uint8_t* d, uint64_t n, uint32_t len, uint32_t* out)
+{
+    for (int pass = 0; pass < 2; ++pass) {
+        RunRing<true, 128, 3>(d, n, len, out, 24);
+        RunRing<true, 128, 4>(d, n, len, out, 16);
+        RunRing1Shapes<128>(d, n, len, out);
+        RunRing1Shapes<256>(d, n, len, out);
+    }
+}
+
 int main(int argc, char** argv)
 {
     const double gib = argc > 1 ? std::atof(argv[1]) : 4.0;
@@ -468,6 +543,10 @@ int main(int argc, char** argv)
     CK(cudaMalloc(&d, n * len));
     CK(cudaMalloc(&out, 64));
     CK(cudaMemset(d, 0x5a, n * len));
+    if (argc > 3 && std::strcmp(argv[3], "ring") == 0) {
+        RunRingComparison(d, n, len, out);
+        return 0;
+    }
     RunPipe<1>("lds_only", out);
     RunPipe<2>("shfl_only", out);
     RunPipe<3>("lds_and_shfl", out);
