@@ -169,6 +169,31 @@ int pire_gpu_run_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uint6
                         const uint32_t* d_start,
                         uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx, void* stream);
 
+/* A batch of streams resumed where each one stopped.  Replaces, for every string i of a batch,
+ *     Pire::Runner(sc, st_i) [.Begin()] .Run(string i) [.End()]                            run.h:365-392
+ * (many texts arriving in pieces at once -- connections, log tails, files read block by block -- each carried on from
+ * the state its last piece ended in).
+ *   Batch   as pire_gpu_run_batch: CSR (d_offsets) or fixed length.  d_order may be NULL; when given it has the
+ *           meaning of pire_gpu_run_batch_ordered (CSR only, n < 2^31; a d_order with d_offsets == NULL is
+ *           PIRE_GPU_EINVAL).
+ *   Start   d_start: n device words, required for n > 0.  d_start[i] is a StateIndex in the reference's numbering and
+ *           string i starts from it (with d_order too: every array is indexed by the original string number).  BEGIN
+ *           steps BeginMark from each string's own start, END steps EndMark after its bytes.  A start >= Size() reads no
+ *           table and yields match 0, mask 0 and state 0xFFFFFFFF, as in pire_gpu_run_string.
+ *   Chain   the d_state_idx of a call made without END is the d_start of the next call, and it may be the same buffer:
+ *           a batch of streams is updated in place round after round with no synchronise in between.
+ *   flags   PIRE_GPU_RUN_BEGIN and/or PIRE_GPU_RUN_END; anything else (PIRE_GPU_RUN_LINES included) is PIRE_GPU_EINVAL,
+ *           as are a NULL d_start and a NULL corpus with non-empty strings.  n == 0 is a no-op.
+ *   Output  as pire_gpu_run_batch (bits past n are 0, nothing past n is written).
+ * The kernel variant is chosen as pire_gpu_run_batch chooses it, AUTO's recorded choice included; PRIV runs PLAIN's
+ * walk.  Asynchronous on `stream`; a host-only handle gets PIRE_GPU_ENODEVICE. */
+int pire_gpu_run_batch_from(const pire_gpu_scanner* sc,
+                            const uint8_t* d_corpus, const uint64_t* d_offsets, const uint32_t* d_order,
+                            uint64_t fixed_len, uint64_t n, uint32_t flags,
+                            const uint32_t* d_start,
+                            uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx,
+                            void* stream);
+
 /* Replaces, per string of a batch,
  *     Pire::LongestPrefix(sc, begin, end, throughBeginMark, throughEndMark)   run.h:277-292
  *     Pire::ShortestPrefix(sc, begin, end, throughBeginMark, throughEndMark)   run.h:294-311

@@ -170,9 +170,27 @@ private:
 // Counterpart of Pire::RunHelper (run.h:365-386) for a device batch.  Results are
 // written to caller-owned device buffers (any may be null); MatchesHost() etc. are
 // conveniences that copy them back through the host entry point.
+// Runner(sc, st) for every string of the batch (pire_gpu_run_batch_from): the start states are n device words, tagged
+// with From() so that a bare pointer is never taken for them, and the state output may be the same buffer, so that a
+// batch of streams is carried on in place round after round:
+//     Runner(gsc, BatchRunner::From(d_state)).Run(piece_k).Launch(nullptr, nullptr, d_state);          // round k
+//     Runner(gsc, BatchRunner::From(d_state)).Run(last).End().Launch(d_bits, d_masks, d_state);        // the last one
 class BatchRunner {
 public:
-    explicit BatchRunner(const Scanner& sc) : Sc(&sc), Flags(0), Ran(false) {}
+    // n device words holding the StateIndex each string starts from (Runner(sc, st), run.h:391-392)
+    struct StartWords {
+        explicit StartWords(const uint32_t* d_words) : Words(d_words) {}
+        const uint32_t* Words;
+    };
+    static StartWords From(const uint32_t* d_start) { return StartWords(d_start); }
+
+    explicit BatchRunner(const Scanner& sc) : Sc(&sc), Start(nullptr), Flags(0), Ran(false) {}
+    BatchRunner(const Scanner& sc, StartWords start) : BatchRunner(sc)
+    {
+        if (!start.Words)
+            throw Error(PIRE_GPU_EINVAL, "BatchRunner::From needs device words");
+        Start = start.Words;
+    }
 
     BatchRunner& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }      // run.h:375
     BatchRunner& End() { Flags |= PIRE_GPU_RUN_END; return *this; }          // run.h:376
@@ -183,6 +201,12 @@ public:
     {
         if (!Ran)
             throw Error(PIRE_GPU_EINVAL, "BatchRunner::Run() was not called");
+        if (Start) {
+            Check(pire_gpu_run_batch_from(Sc->Raw(), Input.Corpus, Input.Offsets, nullptr, Input.FixedLen, Input.Count, Flags, Start,
+                                          d_match_bits, d_accept_masks, d_state_idx, stream),
+                  "pire_gpu_run_batch_from");
+            return;
+        }
         Check(pire_gpu_run_batch(Sc->Raw(), Input.Corpus, Input.Offsets, Input.FixedLen, Input.Count, Flags, d_match_bits,
                                  d_accept_masks, d_state_idx, stream),
               "pire_gpu_run_batch");
@@ -190,12 +214,15 @@ public:
 
 private:
     const Scanner* Sc;
+    const uint32_t* Start;
     Batch Input;
     unsigned Flags;
     bool Ran;
 };
 
 inline BatchRunner Runner(const Scanner& sc) { return BatchRunner(sc); }     // run.h:388-389
+// run.h:391-392, for every string of a batch
+inline BatchRunner Runner(const Scanner& sc, BatchRunner::StartWords start) { return BatchRunner(sc, start); }
 
 // Counterpart of Pire::RunHelper (run.h:365-392) for ONE string resident in HBM, scanned by the whole GPU
 // (pire_gpu_run_string).  Run() may be called many times: the pieces are scanned as one string, the state carried in

@@ -75,6 +75,22 @@ uint32_t ResolveVariant(const pire_gpu_scanner* sc, bool uniform)
     return PIRE_GPU_VARIANT_PLAIN;
 }
 
+uint32_t BatchVariant(const pire_gpu_scanner* sc, bool uniform, uint64_t n)
+{
+    uint32_t variant = ResolveVariant(sc, uniform);
+    if (variant == PIRE_GPU_VARIANT_PRIV && !(uniform && sc->priv_ok))
+        variant = PIRE_GPU_VARIANT_PLAIN;       // the private-row kernel exists for uniform batches only
+    if (variant == PIRE_GPU_VARIANT_LOOK && uniform && sc->variant == PIRE_GPU_VARIANT_AUTO) {
+        // two strings per lane pay when every resident warp gets a pair of units; a smaller batch (a 64 MiB chunk of
+        // the host entry point, say) keeps more warps busy with one string per lane
+        const LaunchPlan& two = sc->plan[PIRE_GPU_VARIANT_LOOK][1];
+        const uint64_t pairs = ((n + 31) / 32 + 1) / 2;
+        if (pairs < (uint64_t) two.grid * (uint64_t) (two.block / 32))
+            variant = PIRE_GPU_VARIANT_LOOK1;
+    }
+    return variant;
+}
+
 namespace {
 
 int Upload(pire_gpu_scanner* sc)
@@ -146,6 +162,8 @@ int Upload(pire_gpu_scanner* sc)
             }
             if (pe != cudaSuccess)
                 return FailCuda(pe, "PlanScan");
+            if (v != kVariantPriv)
+                CUDA_TRY(PlanScan(sc->device, t.hot, t.hot_small, t.priv_rows, v, u != 0, &sc->plan_from[v][u], true));
         }
     return PIRE_GPU_OK;
 }
@@ -315,6 +333,42 @@ int pire_gpu_scanner_set_count_mode(pire_gpu_scanner* sc, uint32_t mode)
     return PIRE_GPU_OK;
 }
 
+// Per-string starts (pire_gpu_run_batch_from): n words of StateIndex, mapped and stepped through BeginMark in the kernels.
+static void SetStarts(const pire_gpu_scanner* sc, ScanArgs* a, const uint32_t* d_start, uint32_t flags)
+{
+    a->starts = d_start;
+    a->new_of_old = sc->dev.new_of_old;
+    a->states = sc->tab.states;
+    a->with_begin = (flags & PIRE_GPU_RUN_BEGIN) ? 1 : 0;
+    a->begin_class = sc->tab.begin_class;
+}
+
+// pire_gpu_run_batch once its arguments are checked; d_start = per-string starts or null
+static int RunBatch(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets, uint64_t fixed_len, uint64_t n,
+                    uint32_t flags, const uint32_t* d_start, uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx,
+                    void* stream)
+{
+    if (n > (1ull << 40))
+        return Fail(PIRE_GPU_EINVAL, "too many strings");
+    CUDA_TRY(cudaSetDevice(sc->device));
+    ScanArgs a;
+    FillArgs(sc, &a, d_corpus, d_offsets, fixed_len, n, flags);
+    a.match_bits = d_match_bits;
+    a.accept_masks = d_accept_masks;
+    a.state_idx = d_state_idx;
+    const bool uniform = IsUniform(d_corpus, d_offsets, fixed_len);
+    uint32_t variant = BatchVariant(sc, uniform, n);
+    const LaunchPlan* plan = &sc->plan[variant][uniform ? 1 : 0];
+    if (d_start) {
+        SetStarts(sc, &a, d_start, flags);
+        if (variant == PIRE_GPU_VARIANT_PRIV)
+            variant = PIRE_GPU_VARIANT_PLAIN;       // no private-row kernel with starts: PLAIN's walk
+        plan = &sc->plan_from[variant][uniform ? 1 : 0];
+    }
+    CUDA_TRY(LaunchScan(a, (int) variant, uniform, *plan, static_cast<cudaStream_t>(stream)));
+    return PIRE_GPU_OK;
+}
+
 int pire_gpu_run_batch(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,
                        uint64_t fixed_len, uint64_t n, uint32_t flags,
                        uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx, void* stream)
@@ -328,28 +382,7 @@ int pire_gpu_run_batch(const pire_gpu_scanner* sc, const uint8_t* d_corpus, cons
         return PIRE_GPU_OK;
     if (!d_corpus && (d_offsets || fixed_len != 0))
         return Fail(PIRE_GPU_EINVAL, "null corpus with non-empty strings");
-    if (n > (1ull << 40))
-        return Fail(PIRE_GPU_EINVAL, "too many strings");
-    CUDA_TRY(cudaSetDevice(sc->device));
-    ScanArgs a;
-    FillArgs(sc, &a, d_corpus, d_offsets, fixed_len, n, flags);
-    a.match_bits = d_match_bits;
-    a.accept_masks = d_accept_masks;
-    a.state_idx = d_state_idx;
-    const bool uniform = IsUniform(d_corpus, d_offsets, fixed_len);
-    uint32_t variant = ResolveVariant(sc, uniform);
-    if (variant == PIRE_GPU_VARIANT_PRIV && !(uniform && sc->priv_ok))
-        variant = PIRE_GPU_VARIANT_PLAIN;       // the private-row kernel exists for uniform batches only
-    if (variant == PIRE_GPU_VARIANT_LOOK && uniform && sc->variant == PIRE_GPU_VARIANT_AUTO) {
-        // two strings per lane pay when every resident warp gets a pair of units; a smaller batch (a 64 MiB chunk of
-        // the host entry point, say) keeps more warps busy with one string per lane
-        const LaunchPlan& two = sc->plan[PIRE_GPU_VARIANT_LOOK][1];
-        const uint64_t pairs = ((n + 31) / 32 + 1) / 2;
-        if (pairs < (uint64_t) two.grid * (uint64_t) (two.block / 32))
-            variant = PIRE_GPU_VARIANT_LOOK1;
-    }
-    CUDA_TRY(LaunchScan(a, (int) variant, uniform, sc->plan[variant][uniform ? 1 : 0], static_cast<cudaStream_t>(stream)));
-    return PIRE_GPU_OK;
+    return RunBatch(sc, d_corpus, d_offsets, fixed_len, n, flags, nullptr, d_match_bits, d_accept_masks, d_state_idx, stream);
 }
 
 static int PrefixOrSuffix(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets, uint64_t fixed_len,
@@ -476,7 +509,30 @@ int pire_gpu_length_order(const uint64_t* d_offsets, uint64_t n, uint32_t* d_ord
 
 static int RunCsr(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets, const uint32_t* d_order,
                   uint64_t n, uint32_t flags, uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx,
-                  void* stream);
+                  void* stream, const uint32_t* d_start = nullptr);
+
+int pire_gpu_run_batch_from(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets, const uint32_t* d_order,
+                            uint64_t fixed_len, uint64_t n, uint32_t flags, const uint32_t* d_start,
+                            uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx, void* stream)
+{
+    int rc = CheckRunnable(sc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_run_batch_from takes PIRE_GPU_RUN_BEGIN and PIRE_GPU_RUN_END only");
+    if (n == 0)
+        return PIRE_GPU_OK;
+    if (!d_start)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_run_batch_from needs n start states");
+    if (!d_corpus && (d_offsets || fixed_len != 0))
+        return Fail(PIRE_GPU_EINVAL, "null corpus with non-empty strings");
+    if (d_order) {
+        if (!d_offsets)
+            return Fail(PIRE_GPU_EINVAL, "an order needs a CSR batch");
+        return RunCsr(sc, d_corpus, d_offsets, d_order, n, flags, d_match_bits, d_accept_masks, d_state_idx, stream, d_start);
+    }
+    return RunBatch(sc, d_corpus, d_offsets, fixed_len, n, flags, d_start, d_match_bits, d_accept_masks, d_state_idx, stream);
+}
 
 int pire_gpu_run_batch_ordered(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,
                                const uint32_t* d_order, uint64_t n, uint32_t flags,
@@ -513,7 +569,7 @@ int pire_gpu_run_lines(const pire_gpu_scanner* sc, const uint8_t* d_text, const 
 
 static int RunCsr(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets, const uint32_t* d_order,
                   uint64_t n, uint32_t flags, uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx,
-                  void* stream)
+                  void* stream, const uint32_t* d_start)
 {
     int rc = CheckRunnable(sc);
     if (rc != PIRE_GPU_OK)
@@ -554,9 +610,10 @@ static int RunCsr(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uin
             a.split_count = counter + 2;
         }
     }
-    uint32_t variant = ResolveVariant(sc, false);
-    if (variant == PIRE_GPU_VARIANT_PRIV)
-        variant = PIRE_GPU_VARIANT_PLAIN;
+    const uint32_t variant = BatchVariant(sc, false, n);
+    const LaunchPlan& plan = d_start ? sc->plan_from[variant][0] : sc->plan[variant][0];
+    if (d_start)
+        SetStarts(sc, &a, d_start, flags);
     if (split && ce == cudaSuccess)
         ce = LaunchSplit(a, (int) variant, sc->device, st);       // the long strings, one per warp; the rest below
     static const bool lines_kernel = [] {
@@ -570,7 +627,7 @@ static int RunCsr(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uin
         if (ce == cudaSuccess)
             ce = LaunchLines(a, (int) variant, sc->device, st);
     } else if (ce == cudaSuccess)
-        ce = LaunchScan(a, (int) variant, false, sc->plan[variant][0], st);
+        ce = LaunchScan(a, (int) variant, false, plan, st);
     if (counter)
         cudaFreeAsync(counter, st);
     if (ce != cudaSuccess)

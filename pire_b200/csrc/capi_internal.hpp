@@ -67,6 +67,7 @@ struct pire_gpu_scanner {
     uint32_t accept_words = 1;      // 32-bit words per accept set: ceil(max(1, regexps) / 32)
     std::vector<uint32_t> hot_order;
     pire_b200::LaunchPlan plan[pire_b200::kVariantSlots][2];          // [variant][uniform]
+    pire_b200::LaunchPlan plan_from[pire_b200::kVariantSlots][2];     // the same for per-string starts (no PRIV)
 
     // Workspaces of the host-buffer entry point: a call takes a free one (or makes one), so concurrent calls on one
     // handle do not serialise; the mutex guards this list only.
@@ -77,6 +78,8 @@ struct pire_gpu_scanner {
 namespace pire_b200 {
 
 uint32_t ResolveVariant(const pire_gpu_scanner* sc, bool uniform = true);
+// the variant a batch of n strings runs (pire_gpu_run_batch, pire_gpu_run_batch_ordered, pire_gpu_run_batch_from)
+uint32_t BatchVariant(const pire_gpu_scanner* sc, bool uniform, uint64_t n);
 bool IsUniform(const uint8_t* corpus, const uint64_t* offsets, uint64_t fixed_len);
 void FillArgs(const pire_gpu_scanner* sc, ScanArgs* a, const uint8_t* corpus, const uint64_t* offsets, uint64_t fixed_len,
               uint64_t n, uint32_t flags);

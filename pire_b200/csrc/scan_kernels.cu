@@ -373,9 +373,12 @@ __device__ __forceinline__ void Chunk16(const Tables& t, LaneState& s, uint4 v)
     }
 }
 
-__device__ __forceinline__ void Report(const ScanArgs& a, const Tables& t, const LaneState& s, uint64_t unit, uint64_t i, bool valid)
+// known = false: the string started from a StateIndex outside the scanner (LaneStart); it reports match 0, mask 0 and
+// state 0xFFFFFFFF whatever its walk did, and stays out of the match ballot.
+__device__ __forceinline__ void Report(const ScanArgs& a, const Tables& t, const LaneState& s, uint64_t unit, uint64_t i, bool valid,
+                                       bool known = true)
 {
-    DeviceFin f = a.fin[FullState(t, s)];
+    DeviceFin f = known ? a.fin[FullState(t, s)] : DeviceFin{0u, 0u};
     unsigned matched = __ballot_sync(0xffffffffu, valid && (f.result >> 31));
     if (a.match_bits && (threadIdx.x & 31) == 0)
         a.match_bits[unit] = matched;
@@ -383,29 +386,66 @@ __device__ __forceinline__ void Report(const ScanArgs& a, const Tables& t, const
         if (a.accept_masks)
             a.accept_masks[i] = f.mask;
         if (a.state_idx)
-            a.state_idx[i] = f.result & 0x7fffffffu;
+            a.state_idx[i] = known ? f.result & 0x7fffffffu : 0xFFFFFFFFu;
     }
 }
 
 // Ordered (length-binned) launches: lane -> string is a permutation, so the match
 // bit goes to its word with an atomic OR (the caller zeroes the bitmap).
-__device__ __forceinline__ void ReportScattered(const ScanArgs& a, const Tables& t, const LaneState& s, uint64_t i, bool valid)
+__device__ __forceinline__ void ReportScattered(const ScanArgs& a, const Tables& t, const LaneState& s, uint64_t i, bool valid,
+                                                bool known = true)
 {
     if (!valid)
         return;
-    DeviceFin f = a.fin[FullState(t, s)];
+    DeviceFin f = known ? a.fin[FullState(t, s)] : DeviceFin{0u, 0u};
     if (a.match_bits && (f.result >> 31))
         atomicOr(&a.match_bits[i >> 5], 1u << (i & 31));
     if (a.accept_masks)
         a.accept_masks[i] = f.mask;
     if (a.state_idx)
-        a.state_idx[i] = f.result & 0x7fffffffu;
+        a.state_idx[i] = known ? f.result & 0x7fffffffu : 0xFFFFFFFFu;
+}
+
+// ---------------------------------------------------------------- starts given by the caller
+
+// One cell of the complete table (global memory / L2).
+__device__ __forceinline__ uint32_t FullCell(const Tables& t, uint32_t s, uint32_t cls)
+{
+    const size_t at = (size_t) s * t.letters + cls;
+    return t.wide ? __ldg(static_cast<const uint32_t*>(t.full) + at) : (uint32_t) __ldg(static_cast<const uint16_t*>(t.full) + at);
+}
+
+// The state a run starts from when the caller gives it as a StateIndex `old` (reference numbering, Runner(sc, st),
+// run.h:391-392): mapped to the new numbering, with BeginMark stepped through the complete table when a.with_begin.  A
+// StateIndex at or above Size() reads no table: `known` is cleared and `start` left as it was (the run goes on from it,
+// and its result is never reported).
+__device__ __forceinline__ void StartFrom(const ScanArgs& a, const Tables& t, uint32_t old, uint32_t& start, bool& known)
+{
+    known = old < a.states;
+    if (known) {
+        start = a.new_of_old[old];
+        if (a.with_begin)
+            start = FullCell(t, start, a.begin_class);
+    }
+}
+
+// The start of string i in a batch kernel: a.start, or with kStarts its own (a.starts[i], pire_gpu_run_batch_from).  A lane
+// past the batch (in_batch false) reads no start.  a.starts may be a.state_idx: every kernel calls this for string i
+// before it reports string i.
+template <bool kStarts>
+__device__ __forceinline__ uint32_t LaneStart(const ScanArgs& a, const Tables& t, uint64_t i, bool in_batch, bool& known)
+{
+    uint32_t start = a.start;
+    known = true;
+    if (kStarts && in_batch)
+        StartFrom(a, t, a.starts[i], start, known);
+    return start;
 }
 
 // ---------------------------------------------------------------- kernels
 
-// Uniform batch: fixed length, length % 32 == 0, corpus 32-byte aligned.
-template <bool kPred>
+// Uniform batch: fixed length, length % 32 == 0, corpus 32-byte aligned.  kStarts: every string from its own start (LaneStart).
+template <bool kPred, bool kStarts>
 __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanUniformKernel(const __grid_constant__ ScanArgs a)
 {
     uint8_t* const smem = pire_b200_smem;
@@ -433,7 +473,8 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanUniformKernel(con
         const uint8_t* p = a.corpus + (valid ? i : a.n - 1) * (uint64_t) len;
 
         LaneState s;
-        SetFull(t, s, a.start);
+        bool known;
+        SetFull(t, s, LaneStart<kStarts>(a, t, i, valid, known));
 
         if (len != 0) {
             // Two register sets in ping-pong: the 32 bytes after the ones being walked are
@@ -461,7 +502,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanUniformKernel(con
                     break;
             }
         }
-        Report(a, t, s, unit, i, valid);
+        Report(a, t, s, unit, i, valid, known);
     }
 }
 
@@ -645,7 +686,7 @@ __device__ __forceinline__ void LookBlock32(const Tables& t, uint32_t& g, uint32
 constexpr int kLookBlock40 = 512;
 constexpr int kLookBlock48 = 640;
 
-template <bool k64, int kRegs, bool kClean = false>
+template <bool k64, int kRegs, bool kClean, bool kStarts>
 __global__ void __maxnreg__(kRegs) ScanUniformLookKernel(const __grid_constant__ ScanArgs a)
 {
     uint8_t* const smem = pire_b200_smem;
@@ -675,11 +716,13 @@ __global__ void __maxnreg__(kRegs) ScanUniformLookKernel(const __grid_constant__
 
     for (uint32_t unit = blockIdx.x * warps_per_block + (threadIdx.x >> 5); unit < units; unit += warps) {
         uint32_t g, prev;
+        bool known;
         {
             const uint64_t i = (uint64_t) unit * 32 + (threadIdx.x & 31);
             const uint8_t* p = a.corpus + (i < a.n ? i : a.n - 1) * (uint64_t) len;
-            prev = a.start;
-            g = a.start < t.H ? a.start : t.H;
+            const uint32_t start = LaneStart<kStarts>(a, t, i, i < a.n, known);
+            prev = start;
+            g = start < t.H ? start : t.H;
             if (blocks != 0) {
                 uint4 a0, a1, b0, b1;
                 LoadStream32(p, a0, a1);
@@ -713,7 +756,7 @@ __global__ void __maxnreg__(kRegs) ScanUniformLookKernel(const __grid_constant__
         LaneState s;
         s.g = t.H;              // Report reads the complete state
         s.cold = g == t.H ? prev : g;
-        Report(a, t, s, unit, i, i < a.n);
+        Report(a, t, s, unit, i, i < a.n, known);
     }
 }
 
@@ -940,7 +983,9 @@ struct RingNext {
     }
 };
 
-__global__ void __launch_bounds__(kRingBlock, 1) ScanUniformLookRingKernel(const __grid_constant__ ScanArgs a)
+// The walk of ScanUniformLookRingKernel, and with kStarts of ScanUniformLookRingFromKernel (each string from its own start).
+template <bool kStarts>
+__device__ __forceinline__ void LookRingScan(const ScanArgs& a)
 {
     uint8_t* const smem = pire_b200_smem;
     SharedView sv = CarveShared(smem, a.hot);
@@ -973,13 +1018,23 @@ __global__ void __launch_bounds__(kRingBlock, 1) ScanUniformLookRingKernel(const
     for (uint32_t pair = blockIdx.x * warps_per_block + (threadIdx.x >> 5); pair < pairs; pair += warps) {
         const bool second = 2 * pair + 1 < units;          // the last pair of an odd batch walks its first unit twice
         uint32_t ga, preva, gb, prevb;
+        bool knowna, knownb;
         {
             const uint64_t ia = (uint64_t) pair * 64 + (threadIdx.x & 31);
             const uint64_t ib = ia + (second ? 32 : 0);
             const uint8_t* pa = a.corpus + (ia < a.n ? ia : a.n - 1) * (uint64_t) len;
             const uint8_t* pb = a.corpus + (ib < a.n ? ib : a.n - 1) * (uint64_t) len;
-            preva = prevb = a.start;
-            ga = gb = a.start < t.H ? a.start : t.H;
+            if constexpr (kStarts) {
+                preva = LaneStart<true>(a, t, ia, ia < a.n, knowna);
+                prevb = LaneStart<true>(a, t, ib, ib < a.n, knownb);
+                ga = preva < t.H ? preva : t.H;
+                gb = prevb < t.H ? prevb : t.H;
+            } else {
+                // as it was before starts existed: the kernel compiles to the same code
+                knowna = knownb = true;
+                preva = prevb = a.start;
+                ga = gb = a.start < t.H ? a.start : t.H;
+            }
             if (blocks != 0) {
                 // Blocks 0..2 of both strings, one commit group per block (empty past the end); block k + 3 refills the
                 // slot of block k as soon as block k is in registers.  No copy reaches past the end of a string: the
@@ -1031,13 +1086,19 @@ __global__ void __launch_bounds__(kRingBlock, 1) ScanUniformLookRingKernel(const
         LaneState s;
         s.g = t.H;
         s.cold = ga == t.H ? preva : ga;
-        Report(a, t, s, 2 * (uint64_t) pair, ia, ia < a.n);
+        Report(a, t, s, 2 * (uint64_t) pair, ia, ia < a.n, knowna);
         if (second) {
             s.cold = gb == t.H ? prevb : gb;
-            Report(a, t, s, 2 * (uint64_t) pair + 1, ia + 32, ia + 32 < a.n);
+            Report(a, t, s, 2 * (uint64_t) pair + 1, ia + 32, ia + 32 < a.n, knownb);
         }
     }
 }
+
+__global__ void __launch_bounds__(kRingBlock, 1) ScanUniformLookRingKernel(const __grid_constant__ ScanArgs a) { LookRingScan<false>(a); }
+
+// The same kernel with per-string starts (pire_gpu_run_batch_from), under a name of its own: the one above is the one
+// that runs without.
+__global__ void __launch_bounds__(kRingBlock, 1) ScanUniformLookRingFromKernel(const __grid_constant__ ScanArgs a) { LookRingScan<true>(a); }
 
 // ---------------------------------------------------------------- LOOK variant, one string per lane, fed from a ring
 //
@@ -1069,7 +1130,7 @@ struct RingNext1 {
     }
 };
 
-template <int kSlots>
+template <int kSlots, bool kStarts>
 __global__ void __launch_bounds__(kRing1Block, 1) ScanUniformLookRing1Kernel(const __grid_constant__ ScanArgs a)
 {
     uint8_t* const smem = pire_b200_smem;
@@ -1101,11 +1162,13 @@ __global__ void __launch_bounds__(kRing1Block, 1) ScanUniformLookRing1Kernel(con
 
     for (uint32_t unit = blockIdx.x * warps_per_block + (threadIdx.x >> 5); unit < units; unit += warps) {
         uint32_t g, prev;
+        bool known;
         {
             const uint64_t i = (uint64_t) unit * 32 + (threadIdx.x & 31);
             const uint8_t* p = a.corpus + (i < a.n ? i : a.n - 1) * (uint64_t) len;
-            prev = a.start;
-            g = a.start < t.H ? a.start : t.H;
+            const uint32_t start = LaneStart<kStarts>(a, t, i, i < a.n, known);
+            prev = start;
+            g = start < t.H ? start : t.H;
             if (blocks != 0) {
                 // Blocks 0..kSlots-1, one commit group per block (empty past the end); block k + kSlots refills the slot
                 // of block k as soon as block k is in registers.  No copy reaches past the end of a string: the last
@@ -1149,7 +1212,7 @@ __global__ void __launch_bounds__(kRing1Block, 1) ScanUniformLookRing1Kernel(con
         LaneState s;
         s.g = t.H;
         s.cold = g == t.H ? prev : g;
-        Report(a, t, s, unit, i, i < a.n);
+        Report(a, t, s, unit, i, i < a.n, known);
     }
 }
 
@@ -1275,7 +1338,7 @@ __device__ __forceinline__ void Chunk16Look(const Tables& t, LaneState& s, uint4
 }
 
 // kMode: 0 plain, 1 exit filter (PRED), 2 exit filter with one byte of look-ahead (LOOK) in the 16-byte body chunks
-template <int kMode>
+template <int kMode, bool kStarts>
 __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) ScanGenericKernel(const __grid_constant__ ScanArgs a)
 {
     constexpr bool kPred = kMode != 0;
@@ -1338,7 +1401,8 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) ScanGenericKernel
         const uint8_t* end = a.corpus + e;
 
         LaneState s;
-        SetFull(t, s, a.start);
+        bool known;
+        SetFull(t, s, LaneStart<kStarts>(a, t, i, valid, known));
 
         // head: up to the first 16-byte boundary.  The bytes come from ONE load of the aligned
         // chunk that holds them (the reference's RunChunk does the same with its head word,
@@ -1412,9 +1476,9 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) ScanGenericKernel
             }
         }
         if (a.order)
-            ReportScattered(a, t, s, i, valid);
+            ReportScattered(a, t, s, i, valid, known);
         else
-            Report(a, t, s, unit, i, valid);
+            Report(a, t, s, unit, i, valid, known);
     }
 }
 
@@ -1550,7 +1614,9 @@ __device__ __forceinline__ void StitchWarp(const Tables& t, const uint8_t* noexi
     }
 }
 
-template <bool kPred>
+// kStarts: the head and lane 0's piece start from the string's own start (LaneStart), the other pieces from the guess as
+// ever; a start outside the scanner rides in bit 32 of the parked string number to the report.
+template <bool kPred, bool kStarts>
 __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanSplitKernel(const __grid_constant__ ScanArgs a)
 {
     uint8_t* const smem = pire_b200_smem;
@@ -1588,7 +1654,8 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanSplitKernel(const
 
         // head, by every lane alike: to the first 32-byte boundary
         LaneState s;
-        SetFull(t, s, a.start);
+        bool known;
+        SetFull(t, s, LaneStart<kStarts>(a, t, i, true, known));
         {
             const uint32_t mis = (uint32_t) (reinterpret_cast<uintptr_t>(p) & 15);
             if (p < end && mis != 0) {
@@ -1613,7 +1680,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanSplitKernel(const
         // the string's bounds wait in shared memory while the pieces are walked: they are the same in every lane and not
         // needed in the loop, which is short of registers (ptxas spilled the loop counter instead)
         if (lane == 0) {
-            parked[0] = i;
+            parked[0] = known ? i : i | (1ull << 32);          // i < 2^31
             parked[1] = reinterpret_cast<uint64_t>(p + 32 * (size_t) blocks_total);
             parked[2] = reinterpret_cast<uint64_t>(end);
         }
@@ -1647,7 +1714,8 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanSplitKernel(const
         }
         if (q < q_end)
             EdgeFast<kPred>(t, s, LoadChunk16(q, buf_lo, buf_hi), (uint32_t) (q_end - q));
-        ReportScattered(a, t, s, parked[0], lane == 0);
+        const uint64_t at = parked[0];
+        ReportScattered(a, t, s, kStarts ? (uint32_t) at : at, lane == 0, !kStarts || (at >> 32) == 0);
         __syncwarp();                      // the next string's bounds replace these
     }
 }
@@ -1692,12 +1760,6 @@ __global__ void SplitCountKernel(const uint64_t* __restrict__ offsets, const uin
 constexpr int kStringBlocksPerSM = 2;           // 64 registers: the walk, the stitch and the rounds without spills
 constexpr uint32_t kStringMinBlocks = 16;       // 32-byte blocks per lane below which the grid gets fewer CTAs
 
-__device__ __forceinline__ uint32_t FullCell(const Tables& t, uint32_t s, uint32_t cls)
-{
-    const size_t at = (size_t) s * t.letters + cls;
-    return t.wide ? __ldg(static_cast<const uint32_t*>(t.full) + at) : (uint32_t) __ldg(static_cast<const uint16_t*>(t.full) + at);
-}
-
 // Where the 32-byte aligned body of the string [p, end) begins: behind the bytes to the next 16-byte boundary and, if
 // that is not a 32-byte one, 16 more.  A string too short for that has no body (the result is not 32-byte aligned).
 __device__ __forceinline__ const uint8_t* StringBody(const uint8_t* p, const uint8_t* end)
@@ -1734,15 +1796,8 @@ __global__ void __launch_bounds__(kBlock, kStringBlocksPerSM) ScanStringKernel(c
     // after a grid.sync(), when every thread has read it.
     uint32_t start = a.start;
     bool valid = true;
-    if (a.start_idx) {
-        const uint32_t old = *a.start_idx;
-        valid = old < a.states;
-        if (valid) {
-            start = a.new_of_old[old];
-            if (a.with_begin)
-                start = FullCell(t, start, a.begin_class);
-        }
-    }
+    if (a.start_idx)
+        StartFrom(a, t, *a.start_idx, start, valid);
     const bool skip = !valid || (start < t.H && sv.noexit[start] != 0);       // multi.h:955-958: no byte leaves it
 
     const uint32_t lane = threadIdx.x & 31;
@@ -3235,10 +3290,10 @@ __global__ void __launch_bounds__(256) SynthMixedFillKernel(uint64_t seed, uint3
     }
 }
 
-template <bool kPred>
-const void* UniformKernelPtr() { return reinterpret_cast<const void*>(&ScanUniformKernel<kPred>); }
-template <int kMode>
-const void* GenericKernelPtr() { return reinterpret_cast<const void*>(&ScanGenericKernel<kMode>); }
+template <bool kPred, bool kStarts = false>
+const void* UniformKernelPtr() { return reinterpret_cast<const void*>(&ScanUniformKernel<kPred, kStarts>); }
+template <int kMode, bool kStarts = false>
+const void* GenericKernelPtr() { return reinterpret_cast<const void*>(&ScanGenericKernel<kMode, kStarts>); }
 
 int LookRegs()
 {
@@ -3294,12 +3349,34 @@ bool LookRing()
 
 // The one-string ring kernel keeps 8 slots per string in 16 warps; PIRE_B200_LOOK_RING1_SLOTS=6 selects 6 slots in 24
 // warps, the same 144 KB of ring per SM as the two-string kernel (experiments).
-const void* KernelFor(int variant, bool uniform)
+// With per-string starts (pire_gpu_run_batch_from) every variant has one kernel, whatever the experiment switches above
+// say: the default shapes, 48 registers for the one-string look-ahead kernel and the ring for LOOK.  PRIV is run as PLAIN
+// by the caller.
+const void* StartsKernelFor(int variant, bool uniform)
 {
+    if (variant == kVariantLookRing1 && uniform)
+        return reinterpret_cast<const void*>(&ScanUniformLookRing1Kernel<kRing1Slots, true>);
+    if (variant == kVariantLook && uniform)
+        return reinterpret_cast<const void*>(&ScanUniformLookRingFromKernel);
+    if (variant == kVariantLook1 && uniform)
+        return reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 48, true, true>);
+    if (variant == kVariantLook64 && uniform)
+        return reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 48, false, true>);
+    if (uniform)
+        return variant == kVariantPred ? UniformKernelPtr<true, true>() : UniformKernelPtr<false, true>();
+    if (variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1 || variant == kVariantLookRing1)
+        return GenericKernelPtr<2, true>();
+    return variant == kVariantPred ? GenericKernelPtr<1, true>() : GenericKernelPtr<0, true>();
+}
+
+const void* KernelFor(int variant, bool uniform, bool starts = false)
+{
+    if (starts)
+        return StartsKernelFor(variant, uniform);
     if (variant == kVariantPriv && uniform)
         return reinterpret_cast<const void*>(&ScanUniformPrivKernel);
     if (variant == kVariantLookRing1 && uniform)
-        return reinterpret_cast<const void*>(&ScanUniformLookRing1Kernel<kRing1Slots>);
+        return reinterpret_cast<const void*>(&ScanUniformLookRing1Kernel<kRing1Slots, false>);
     if (variant == kVariantLook && uniform && LookIlp() == 2 && LookRing())
         return reinterpret_cast<const void*>(&ScanUniformLookRingKernel);
     if (variant == kVariantLook && uniform && LookIlp() == 2)
@@ -3307,14 +3384,14 @@ const void* KernelFor(int variant, bool uniform)
                : LookIlpRegs() == 80 ? reinterpret_cast<const void*>(&ScanUniformLook2Kernel<80>)
                                      : reinterpret_cast<const void*>(&ScanUniformLook2Kernel<72>);
     if ((variant == kVariantLook || variant == kVariantLook1) && uniform && LookClean())
-        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 48, true>)
-                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 40, true>);
+        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 48, true, false>)
+                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 40, true, false>);
     if ((variant == kVariantLook || variant == kVariantLook1) && uniform)
-        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 48>)
-                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 40>);
+        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 48, false, false>)
+                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 40, false, false>);
     if (variant == kVariantLook64 && uniform)
-        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 48>)
-                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 40>);
+        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 48, false, false>)
+                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 40, false, false>);
     if (uniform)
         return variant == kVariantPred ? UniformKernelPtr<true>() : UniformKernelPtr<false>();
     if (variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1 || variant == kVariantLookRing1)
@@ -3338,21 +3415,23 @@ cudaError_t PrepareScanKernels(int device)
         return err;
     for (int variant : {(int) kVariantPlain, (int) kVariantPred, (int) kVariantPriv, (int) kVariantLook, (int) kVariantLook64, (int) kVariantLook1,
                         (int) kVariantLookRing1})
-        for (bool uniform : {false, true}) {
-            err = cudaFuncSetAttribute(KernelFor(variant, uniform), cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
-            if (err != cudaSuccess)
-                return err;
-            // three CTAs of ~75 KB each per SM: ask for the largest shared-memory carve-out (kernels without a
-            // blocks-per-SM launch bound would otherwise get a smaller one and run two CTAs)
-            err = cudaFuncSetAttribute(KernelFor(variant, uniform), cudaFuncAttributePreferredSharedMemoryCarveout,
-                                       cudaSharedmemCarveoutMaxShared);
-            if (err != cudaSuccess)
-                return err;
-        }
+        for (bool uniform : {false, true})
+            for (bool starts : {false, true}) {
+                err = cudaFuncSetAttribute(KernelFor(variant, uniform, starts), cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+                if (err != cudaSuccess)
+                    return err;
+                // three CTAs of ~75 KB each per SM: ask for the largest shared-memory carve-out (kernels without a
+                // blocks-per-SM launch bound would otherwise get a smaller one and run two CTAs)
+                err = cudaFuncSetAttribute(KernelFor(variant, uniform, starts), cudaFuncAttributePreferredSharedMemoryCarveout,
+                                           cudaSharedmemCarveoutMaxShared);
+                if (err != cudaSuccess)
+                    return err;
+            }
     return cudaSuccess;
 }
 
-cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv_rows, int variant, bool uniform, LaunchPlan* plan)
+cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv_rows, int variant, bool uniform, LaunchPlan* plan,
+                     bool starts)
 {
     const bool priv = variant == kVariantPriv && uniform;
     const bool look = variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1;
@@ -3369,8 +3448,12 @@ cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv
     }
     if (variant == kVariantLookRing1 && uniform)
         plan->block = kRing1Block;
+    // the kernels with per-string starts have the default shapes (StartsKernelFor)
+    const bool ring = variant == kVariantLook && uniform && (starts || (LookIlp() == 2 && LookRing()));
+    if (starts && look && uniform)
+        plan->block = ring ? kRingBlock : kLookBlock48;
     plan->shared = priv ? ScanSharedBytes(hot_small, priv_rows) : uniform ? ScanSharedBytes(hot, 0) : GenericSharedBytes(hot);
-    if (variant == kVariantLook && uniform && LookIlp() == 2 && LookRing())
+    if (ring)
         plan->shared += (size_t) (plan->block / 32) * kRingWarpBytes;         // every warp's ring after the tables
     if (variant == kVariantLookRing1 && uniform)
         plan->shared += (size_t) (plan->block / 32) * kRing1Slots * kRing1SlotBytes;      // every warp's ring after the tables
@@ -3378,7 +3461,7 @@ cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv
     cudaError_t err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     if (err != cudaSuccess)
         return err;
-    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, KernelFor(variant, uniform), plan->block, plan->shared);
+    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, KernelFor(variant, uniform, starts), plan->block, plan->shared);
     if (err != cudaSuccess)
         return err;
     if (per_sm < 1)
@@ -3393,14 +3476,15 @@ cudaError_t LaunchScan(const ScanArgs& a, int variant, bool uniform, const Launc
 {
     if (a.n == 0)
         return cudaSuccess;
+    const bool starts = a.starts != nullptr;
     uint64_t units = (a.n + 31) / 32;
-    if (variant == kVariantLook && uniform && LookIlp() == 2)
-        units = (units + 1) / 2;              // a warp of ScanUniformLook2Kernel / ScanUniformLookRingKernel takes two units at a time
+    if (variant == kVariantLook && uniform && (starts || LookIlp() == 2))
+        units = (units + 1) / 2;              // a warp of ScanUniformLook2Kernel / ScanUniformLookRing[From]Kernel takes two units at a time
     const uint64_t warps_per_block = (uint64_t) plan.block / 32;
     uint64_t want = (units + warps_per_block - 1) / warps_per_block;
     int grid = (int) (want < (uint64_t) plan.grid ? want : (uint64_t) plan.grid);
     void* args[] = {const_cast<ScanArgs*>(&a)};
-    cudaError_t err = cudaLaunchKernel(KernelFor(variant, uniform), dim3(grid), dim3(plan.block), args, plan.shared, stream);
+    cudaError_t err = cudaLaunchKernel(KernelFor(variant, uniform, starts), dim3(grid), dim3(plan.block), args, plan.shared, stream);
     if (err == cudaSuccess)
         g_launches.fetch_add(1, std::memory_order_relaxed);
     return err;
@@ -3425,8 +3509,10 @@ cudaError_t LaunchSplit(const ScanArgs& a, int variant, int device, cudaStream_t
         const char* env = getenv("PIRE_B200_SPLIT_PREFETCH");     // blocks of 32 bytes between the walk and its L2 prefetch; 0 = none
         return env ? (uint32_t) atoi(env) : 0u;
     }();
-    const void* fn = variant == kVariantPlain ? reinterpret_cast<const void*>(&ScanSplitKernel<false>)
-                                              : reinterpret_cast<const void*>(&ScanSplitKernel<true>);
+    const void* fn = a.starts ? (variant == kVariantPlain ? reinterpret_cast<const void*>(&ScanSplitKernel<false, true>)
+                                                          : reinterpret_cast<const void*>(&ScanSplitKernel<true, true>))
+                              : (variant == kVariantPlain ? reinterpret_cast<const void*>(&ScanSplitKernel<false, false>)
+                                                          : reinterpret_cast<const void*>(&ScanSplitKernel<true, false>));
     const size_t shared = ScanSharedBytes(a.hot, 0) + kSplitMarkBytes + kWarpsPerBlock * 32;
     int optin = 0, sms = 0, per_sm = 0;
     err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);

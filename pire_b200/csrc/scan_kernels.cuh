@@ -74,6 +74,10 @@ struct ScanArgs {
     uint32_t states;             // Size(): a start_idx at or above it is out of range
     uint32_t* string_ends;       // scratch: 2 x warps of the grid, each warp's end state per stitching round
     unsigned int* string_rounds; // scratch: 3 counters of changed warps, zeroed before the launch
+    // per-string starts (pire_gpu_run_batch_from): string i starts from the StateIndex starts[i] (reference numbering),
+    // mapped through new_of_old, BeginMark stepped when with_begin; one at or above `states` reports (0, 0, 0xFFFFFFFF).
+    // starts may be state_idx: every kernel reads string i's start before it writes string i's state
+    const uint32_t* starts;      // n words, or null: every string starts from `start`
 };
 
 struct LaunchPlan {
@@ -95,7 +99,11 @@ constexpr int kVariantSlots = 8;      // size of per-variant arrays (variant ids
 
 size_t ScanSharedBytes(uint32_t hot, uint32_t priv_rows);
 cudaError_t PrepareScanKernels(int device);                       // raises the dynamic smem limit
-cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv_rows, int variant, bool uniform, LaunchPlan* plan);
+// starts: the plan of the kernel a launch with a.starts runs (the same as without, except for LOOK on uniform batches,
+// which then always runs the two-string ring kernel)
+cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv_rows, int variant, bool uniform, LaunchPlan* plan,
+                     bool starts = false);
+// a.starts selects the kernels that start every string from its own state
 cudaError_t LaunchScan(const ScanArgs& a, int variant, bool uniform, const LaunchPlan& plan, cudaStream_t stream);
 // CSR batches of short strings (lines of text): lanes pull strings dynamically; a.match_bits must be zeroed
 cudaError_t LaunchLines(const ScanArgs& a, int variant, int device, cudaStream_t stream);

@@ -199,5 +199,34 @@ torch.cuda.synchronize()
 assert (np.unpackbits(ball.cpu().numpy().view(np.uint8), bitorder="little")[:1024 + 7] == r.Matches().astype(np.uint8)).all()
 comm.close()
 print("ok accept sets, host streaming, sharded(1)", flush=True)
+# per-string starts (pire_gpu_run_batch_from), chained in place through the state buffer: a uniform batch (the two-string
+# ring kernel and the one-string ring kernel, some starts outside the scanner) and an ordered CSR batch with strings long
+# enough for the split kernel; the results against one run over the whole strings
+from string_oracle import run_from
+img = W.load_image("glue10")
+orc = Oracle(img)
+sc = P.Scanner(img, 0)
+rng = np.random.default_rng(13)
+n, half = 64 * 3 + 5, 128
+whole = rng.choice(np.frombuffer(b"GET error timeout https:// ab(5)", np.uint8), size=(n, 2 * half))
+for variant in (N.VARIANT_LOOK, N.VARIANT_LOOK_RING1):
+    sc.set_variant(variant)
+    st = torch.full((n,), sc.Initialize(), dtype=torch.int32, device=dev)
+    st[7] = sc.Size()
+    for k, flags in ((0, N.RUN_BEGIN), (1, N.RUN_END)):
+        piece = torch.from_numpy(np.ascontiguousarray(whole[:, k * half:(k + 1) * half]).reshape(-1)).to(dev)
+        sc.run_batch(P.Batch(piece, fixed_len=half, n=n), flags, None, None, st, start_idx=st)
+    got = st.cpu().numpy().view(np.uint32)
+    want = [run_from(orc, whole[i], sc.Size() if i == 7 else sc.Initialize(), True, True)[2] for i in range(n)]
+    assert (got == np.array(want, np.uint32)).all(), variant
+strings = [bytes(rng.choice(np.frombuffer(b"GET error timeout ab", np.uint8), size=int(k))) for k in [9000, 20000] + list(rng.integers(0, 600, size=100))]
+bb = P.Batch.from_strings(strings).bin_by_length()
+starts = rng.integers(0, sc.Size(), size=len(strings))
+st = torch.from_numpy(starts.astype(np.int32)).to(dev)
+sc.set_variant(N.VARIANT_PRED)
+sc.run_batch(bb, N.RUN_BEGIN | N.RUN_END, None, None, st, start_idx=st)
+want = [run_from(orc, np.frombuffer(s, np.uint8), int(x), True, True)[2] for s, x in zip(strings, starts)]
+assert (st.cpu().numpy().view(np.uint32) == np.array(want, np.uint32)).all()
+print("ok run_batch_from", flush=True)
 torch.cuda.synchronize()
 print("sanitize_run done, launches:", N.lib.pire_gpu_launch_count())
