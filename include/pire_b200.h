@@ -252,6 +252,35 @@ int pire_gpu_count_batch(const pire_gpu_scanner* sc,
                          uint64_t fixed_len, uint64_t n, uint32_t flags,
                          uint32_t* d_counts, uint32_t* d_match_bits, void* stream);
 
+/* HalfFinalScanner counts of one long string with the whole GPU ("how many times does each pattern occur in this
+ * file").  Replaces, for one string resident in HBM, the driver of tests/count_ut.cpp:54-63 with the state carried
+ * across calls the way a HalfFinalScanner::State is:
+ *     [sc.Initialize(st);]  [Pire::Step(sc, st, BeginMark);]  Pire::Run(sc, st, begin, end);  [Pire::Step(sc, st, EndMark);]
+ * The string is cut into pieces and stitched as in pire_gpu_run_string, then every piece is counted from its true start.
+ *   Input   d_text[0 .. n_bytes), any length (0 included; d_text may then be NULL), any alignment, past 4 GiB too.
+ *   flags   PIRE_GPU_RUN_BEGIN steps BeginMark and counts the state it reaches; PIRE_GPU_RUN_END steps EndMark and
+ *           counts the state it reaches.  Anything else is PIRE_GPU_EINVAL.
+ *   Start   d_start == NULL: Initialize(), whose TakeAction is counted (half_final.h:136-141), as in
+ *           pire_gpu_count_batch.  Otherwise d_start points to ONE device word holding a StateIndex in the reference's
+ *           numbering; the run resumes from it and does NOT count it again (the call that reached it counted it).  A
+ *           start >= Size() adds nothing and yields match 0 and state 0xFFFFFFFF, as in pire_gpu_run_string.
+ *   Counts  d_counts (required): max(1, RegexpsCount()) u64 words that the call ADDS to -- unlike pire_gpu_count_batch,
+ *           whose u32 rows are overwritten.  The caller zeroes them before the first call.  64 bits because one string
+ *           can be longer than 2^32 bytes and a state can list a regexp more than once.
+ *   Chain   the d_state_idx of a call made without END is the d_start of the next call, and it may be the same word;
+ *           d_counts may be the same buffer.  A text arriving in chunks is counted with no synchronise in between
+ *           (BEGIN on the first call, END on the last), and the result equals one call over the concatenated text.
+ *   Output  each may be NULL: d_match_bits[0] = Final() of the last state (the whole word: bit 0, the others 0),
+ *           d_state_idx[0] = its StateIndex (after End() with END).  Nothing else is written.
+ * pire_gpu_scanner_set_count_mode is honoured; the results are identical in every mode.  Whenever the counts fit in 32
+ * bits they equal pire_gpu_count_batch's with n = 1 (CSR) on the same bytes; match and state always equal
+ * pire_gpu_run_string's.  A NULL d_counts and a NULL d_text with n_bytes > 0 are PIRE_GPU_EINVAL; a host-only handle
+ * gets PIRE_GPU_ENODEVICE.  Asynchronous on `stream`; re-entrant across streams on one handle (per-call scratch).  It
+ * costs about pire_gpu_run_string plus one more walk of the bytes, and shares its worst case (DESIGN.md 4). */
+int pire_gpu_count_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uint64_t n_bytes, uint32_t flags,
+                          const uint32_t* d_start, uint64_t* d_counts,
+                          uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
+
 /* The step before the path for line-oriented input (samples/pigrep/pigrep.cpp:38-45 calls
  * std::getline and then Runner(sc).Begin().Run(line).End() per line).
  * pire_gpu_split_lines finds the lines of a newline-delimited text resident in HBM:

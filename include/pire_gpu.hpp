@@ -283,6 +283,60 @@ private:
     bool Ran;
 };
 
+// A Pire::HalfFinalScanner run over ONE string resident in HBM, counted by the whole GPU (pire_gpu_count_string):
+// StringRunner's shape, with the counters of HalfFinalScanner::State.  Run() may be called many times: the pieces are
+// counted as one string, the state carried in the caller-owned device word d_state and the counts ADDED to the
+// caller-owned device array d_counts (max(1, RegexpsCount()) u64, zeroed by the caller before the first call), so
+// chained calls do not synchronise.  After the stream is synchronised, d_counts[r] is State::Result(r)
+// (half_final.h:88-90), *d_state the StateIndex reached and d_match_bits[0] bit 0 Final().  (This header needs no CUDA
+// runtime, so reading the device words is the caller's.)
+//     StringCounter c(gsc, d_counts, d_state);                                 // Initialize(), counted
+//     StringCounter c(gsc, StringCounter::From(d_start), d_counts, d_state);   // resumed from st (not counted again)
+//     c.Begin().Run(d_a, n_a).Run(d_b, n_b).End();
+class StringCounter {
+public:
+    using StartWord = StringRunner::StartWord;
+    static StartWord From(const uint32_t* d_start) { return StartWord(d_start); }
+
+    StringCounter(const Scanner& sc, uint64_t* d_counts, uint32_t* d_state, uint32_t* d_match_bits = nullptr, void* stream = nullptr)
+        : Sc(&sc), Start(nullptr), Counts(d_counts), State(d_state), Bits(d_match_bits), Stream(stream), Flags(0), Ran(false)
+    {
+        if (!d_counts || !d_state)
+            throw Error(PIRE_GPU_EINVAL, "StringCounter needs device words for its counters and its state");
+    }
+    // start.Word may be d_state: the state is then updated in place
+    StringCounter(const Scanner& sc, StartWord start, uint64_t* d_counts, uint32_t* d_state, uint32_t* d_match_bits = nullptr,
+                  void* stream = nullptr)
+        : StringCounter(sc, d_counts, d_state, d_match_bits, stream)
+    {
+        if (!start.Word)
+            throw Error(PIRE_GPU_EINVAL, "StringCounter::From needs a device word");
+        Start = start.Word;
+    }
+
+    StringCounter& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }
+    StringCounter& Run(const uint8_t* d_text, uint64_t n) { Launch(d_text, n, 0); return *this; }
+    StringCounter& End() { Launch(nullptr, 0, PIRE_GPU_RUN_END); return *this; }
+
+private:
+    void Launch(const uint8_t* d_text, uint64_t n, unsigned end)
+    {
+        Check(pire_gpu_count_string(Sc->Raw(), d_text, n, Flags | end, Ran ? State : Start, Counts, Bits, State, Stream),
+              "pire_gpu_count_string");
+        Flags = 0;
+        Ran = true;
+    }
+
+    const Scanner* Sc;
+    const uint32_t* Start;
+    uint64_t* Counts;
+    uint32_t* State;
+    uint32_t* Bits;
+    void* Stream;
+    unsigned Flags;
+    bool Ran;
+};
+
 // AcceptedRegexps for scanners with more than 32 regexps: rows of AcceptWords(sc) words, bit r of row i set iff
 // regexp r is accepted by the state string i stopped in (d_state_idx from BatchRunner::Launch).
 inline uint32_t AcceptWords(const Scanner& sc) { return pire_gpu_accept_words(sc.Raw()); }

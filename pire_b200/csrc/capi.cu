@@ -664,6 +664,46 @@ int pire_gpu_run_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uint6
     return PIRE_GPU_OK;
 }
 
+int pire_gpu_count_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uint64_t n_bytes, uint32_t flags,
+                          const uint32_t* d_start, uint64_t* d_counts, uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream)
+{
+    int rc = CheckRunnable(sc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_count_string takes PIRE_GPU_RUN_BEGIN and PIRE_GPU_RUN_END only");
+    if (!d_counts)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_count_string needs max(1, regexps) u64 counters");
+    if (!d_text && n_bytes)
+        return Fail(PIRE_GPU_EINVAL, "null text with n_bytes > 0");
+    CUDA_TRY(cudaSetDevice(sc->device));
+    ScanArgs a;
+    FillArgs(sc, &a, d_text, nullptr, n_bytes, 1, flags);
+    a.start_idx = d_start;
+    a.new_of_old = sc->dev.new_of_old;
+    a.states = sc->tab.states;
+    a.with_begin = (flags & PIRE_GPU_RUN_BEGIN) ? 1 : 0;
+    a.begin_class = sc->tab.begin_class;
+    a.match_bits = d_match_bits;
+    a.state_idx = d_state_idx;
+    // the counting fields of pire_gpu_count_batch, count mode included
+    a.flags = sc->dev.flags;
+    a.end_class = sc->tab.end_class;
+    a.through_end = (flags & PIRE_GPU_RUN_END) ? 1 : 0;
+    a.acc_begin = sc->dev.acc_begin;
+    a.acc_ids = sc->dev.acc_ids;
+    a.first_final_hot = sc->tab.first_final_hot;
+    a.initial = sc->tab.initial;
+    a.regexps = sc->dfa.regexps ? sc->dfa.regexps : 1;
+    a.weights = sc->dev.weights;
+    a.count_words = sc->count_mode == 1 ? 0 : sc->tab.count_words;
+    a.count_always = (sc->count_mode == 3 || (sc->count_mode == 0 && sc->final_share > 0.025)) ? 1 : 0;
+    a.counts64 = reinterpret_cast<unsigned long long*>(d_counts);
+    a.count_rows = a.regexps <= kCountRowsMax ? 1 : 0;
+    CUDA_TRY(LaunchCountString(a, sc->device, static_cast<cudaStream_t>(stream)));
+    return PIRE_GPU_OK;
+}
+
 int pire_gpu_scanner_tune(pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,
                           uint64_t fixed_len, uint64_t n_sample, uint32_t flags, void* stream)
 {

@@ -1772,6 +1772,43 @@ __device__ __forceinline__ const uint8_t* StringBody(const uint8_t* p, const uin
     return p;
 }
 
+// Both levels of the stitch for the lane's piece (`my_blocks` blocks at `piece`, walked from the guess by WalkPiece; the
+// grid's first lane from first_start), in ScanStringKernel and CountStringKernel: StitchWarp inside the warp, then the
+// rounds over the grid.  Ends after the last grid.sync() with start_full / end_full the true states at the start and at
+// the end of the lane's piece.  A macro over the kernels' own variables, not a function: the same code as a
+// __forceinline__ function changed ScanStringKernel's register allocation (8 bytes of spills), a macro leaves its SASS as
+// it was.
+#define PIRE_B200_STITCH_GRID(kPred)                                                                                           \
+    do {                                                                                                                       \
+        /* level 1: the warp's own pieces, lane 0 keeping its start */                                                         \
+        StitchWarp<kPred>(t, sv.noexit, __shfl_sync(0xffffffffu, start_full, 0), lane, piece, my_blocks, per_mark, marks,      \
+                          head0, head1, head_fresh, start_full, end_full);                                                     \
+        if (lane == 31)                                                                                                        \
+            __stcg(a.string_ends + warp, end_full);                                                                            \
+        grid.sync();                                                                                                           \
+        /* level 2: rounds over the grid.  Round r reads ends[(r-1) & 1], writes ends[r & 1] and counts its changes in       \
+           counter[r % 3]; the counter of the next round is cleared in this one (its last readers finished two rounds ago) */ \
+        for (uint32_t r = 1;; ++r) {                                                                                           \
+            const uint32_t* const in = a.string_ends + ((r - 1) & 1) * warps;                                                  \
+            uint32_t* const out = a.string_ends + (r & 1) * warps;                                                             \
+            const uint32_t want = warp == 0 ? first_start : __ldcg(in + warp - 1);                                             \
+            if (want != __shfl_sync(0xffffffffu, start_full, 0)) {                                                             \
+                bool no_head = false; /* the prefetched first block served level 1; later rounds load it again */             \
+                StitchWarp<kPred>(t, sv.noexit, want, lane, piece, my_blocks, per_mark, marks, make_uint4(0, 0, 0, 0),         \
+                                  make_uint4(0, 0, 0, 0), no_head, start_full, end_full);                                      \
+                if (lane == 0)                                                                                                 \
+                    atomicAdd(a.string_rounds + r % 3, 1u);                                                                    \
+            }                                                                                                                  \
+            if (lane == 31)                                                                                                    \
+                __stcg(out + warp, end_full);                                                                                  \
+            if (me == 0)                                                                                                       \
+                __stcg(a.string_rounds + (r + 1) % 3, 0u);                                                                     \
+            grid.sync();                                                                                                       \
+            if (__ldcg(a.string_rounds + r % 3) == 0)                                                                          \
+                break;                                                                                                         \
+        }                                                                                                                      \
+    } while (0)
+
 template <bool kPred>
 __global__ void __launch_bounds__(kBlock, kStringBlocksPerSM) ScanStringKernel(const __grid_constant__ ScanArgs a)
 {
@@ -1846,33 +1883,7 @@ __global__ void __launch_bounds__(kBlock, kStringBlocksPerSM) ScanStringKernel(c
         bool head_fresh = my_blocks != 0;
         if (head_fresh)
             LoadStream32P(piece, head0, head1);
-        // level 1: the warp's own pieces, lane 0 keeping its start
-        StitchWarp<kPred>(t, sv.noexit, __shfl_sync(0xffffffffu, start_full, 0), lane, piece, my_blocks, per_mark, marks, head0,
-                          head1, head_fresh, start_full, end_full);
-        if (lane == 31)
-            __stcg(a.string_ends + warp, end_full);
-        grid.sync();
-        // level 2: rounds over the grid.  Round r reads ends[(r-1) & 1], writes ends[r & 1] and counts its changes in
-        // counter[r % 3]; the counter of the next round is cleared in this one (its last readers finished two rounds ago).
-        for (uint32_t r = 1;; ++r) {
-            const uint32_t* const in = a.string_ends + ((r - 1) & 1) * warps;
-            uint32_t* const out = a.string_ends + (r & 1) * warps;
-            const uint32_t want = warp == 0 ? first_start : __ldcg(in + warp - 1);
-            if (want != __shfl_sync(0xffffffffu, start_full, 0)) {
-                bool no_head = false;          // the prefetched first block served level 1; later rounds load it again
-                StitchWarp<kPred>(t, sv.noexit, want, lane, piece, my_blocks, per_mark, marks, make_uint4(0, 0, 0, 0),
-                                  make_uint4(0, 0, 0, 0), no_head, start_full, end_full);
-                if (lane == 0)
-                    atomicAdd(a.string_rounds + r % 3, 1u);
-            }
-            if (lane == 31)
-                __stcg(out + warp, end_full);
-            if (me == 0)
-                __stcg(a.string_rounds + (r + 1) % 3, 0u);
-            grid.sync();
-            if (__ldcg(a.string_rounds + r % 3) == 0)
-                break;
-        }
+        PIRE_B200_STITCH_GRID(kPred);
     } else {
         grid.sync();
     }
@@ -2886,16 +2897,37 @@ __global__ void __maxnreg__(48) PrefixUniformKernel(const __grid_constant__ Scan
 // 16 steps landed in a final state or left the hot rows; if not, the chunk costs what a plain scan costs.
 // When a sample showed final states to be frequent (kAlways) that first pass is skipped and every chunk
 // is counted.
-template <int kWords>
+//
+// Where a lane's counts go (Row): the batch kernel's lane-private row of u32 in global memory, or for one string over the
+// grid (CountStringKernel) its warp's row of u32 in shared memory, shared by 32 lanes (atomics), or -- too many regexps
+// for such rows -- the caller's u64 counters in global memory.
+struct WarpRow {
+    uint32_t* shared;               // the warp's row, or null
+    unsigned long long* global;     // used when `shared` is null
+};
+
+__device__ __forceinline__ void AddTo(uint32_t* row, uint32_t id, uint32_t add) { row[id] += add; }
+
+__device__ __forceinline__ void AddTo(const WarpRow& row, uint32_t id, uint32_t add)
+{
+    if (add == 0)
+        return;
+    if (row.shared)
+        atomicAdd(row.shared + id, add);
+    else
+        atomicAdd(row.global + id, (unsigned long long) add);
+}
+
+template <int kWords, class Row = uint32_t*>
 struct Counter {
     uint64_t a8[kWords];            // 8 x 8 bits: at most 16 steps x 15 per field between Widen() calls
     uint64_t even[kWords], odd[kWords];   // 4 x 16 bits each
     uint32_t groups;
-    uint32_t* row;
+    Row row;
     const uint64_t* hot_w;          // shared: (H + 1) * kWords words, the sink's are zero
     const uint64_t* all_w;          // global: states * kWords
 
-    __device__ __forceinline__ void Reset(const ScanArgs& a, const uint64_t* hot_weights, uint32_t* r)
+    __device__ __forceinline__ void Reset(const ScanArgs& a, const uint64_t* hot_weights, Row r)
     {
 #pragma unroll
         for (int j = 0; j < kWords; ++j)
@@ -2919,7 +2951,7 @@ struct Counter {
                 const uint64_t src = (f & 1) ? odd[j] : even[j];
                 const uint32_t add = (uint32_t) (src >> (16 * (f >> 1))) & 0xffffu;
                 if (add)
-                    row[j * 8 + f] += add;
+                    AddTo(row, j * 8 + f, add);
             }
             even[j] = odd[j] = 0;
         }
@@ -2945,12 +2977,12 @@ struct Counter {
     __device__ __forceinline__ void Finish(uint32_t regexps) { Flush(regexps); }
 };
 
-template <>
-struct Counter<0> {
+template <class Row>
+struct Counter<0, Row> {
     uint32_t c0, c1, c2, c3;
-    uint32_t* row;
+    Row row;
 
-    __device__ __forceinline__ void Reset(const ScanArgs&, const uint64_t*, uint32_t* r)
+    __device__ __forceinline__ void Reset(const ScanArgs&, const uint64_t*, Row r)
     {
         c0 = c1 = c2 = c3 = 0;
         row = r;
@@ -2969,22 +3001,22 @@ struct Counter<0> {
             c2 += id == 2;
             c3 += id == 3;
             if (id >= 4)
-                row[id] += 1;
+                AddTo(row, id, 1);
         }
     }
     __device__ __forceinline__ void EndGroup(uint32_t) {}
     __device__ __forceinline__ void Discard() {}
     __device__ __forceinline__ void Finish(uint32_t regexps)
     {
-        row[0] += c0;
-        if (regexps > 1) row[1] += c1;
-        if (regexps > 2) row[2] += c2;
-        if (regexps > 3) row[3] += c3;
+        AddTo(row, 0, c0);
+        if (regexps > 1) AddTo(row, 1, c1);
+        if (regexps > 2) AddTo(row, 2, c2);
+        if (regexps > 3) AddTo(row, 3, c3);
     }
 };
 
-template <int kWords, bool kAlways>
-__device__ __forceinline__ void CountChunk16(const ScanArgs& a, const Tables& t, LaneState& s, uint4 v, Counter<kWords>& c)
+template <int kWords, bool kAlways, class Row>
+__device__ __forceinline__ void CountChunk16(const ScanArgs& a, const Tables& t, LaneState& s, uint4 v, Counter<kWords, Row>& c)
 {
     const uint32_t before = s.g;
     if (!kAlways || kWords == 0) {
@@ -3194,6 +3226,193 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) CountKernel(const
             a.match_bits[unit] = matched;
         if (valid)
             c.Finish(a.regexps);
+    }
+}
+
+// ---------------------------------------------------------------- counting one string over the whole grid
+//
+// HalfFinalScanner counts of one string (pire_gpu_count_string).  The counts depend on every state the walk enters, so
+// each lane needs the true state at the start of its piece; the kernel runs in two phases in one cooperative launch.
+//   1. Locate: ScanStringKernel's head, pieces, walk and stitch (WalkPiece, PIRE_B200_STITCH_GRID), with the plain walk.  After its last
+//      grid.sync() every lane knows the true state at the start of its piece.
+//   2. Count: every lane walks its piece again from there with CountChunk16, 32-byte loads one block ahead in registers
+//      (CountKernel's uniform body).  The head (before the first 32-byte boundary), Initialize() and BeginMark are counted
+//      by the grid's first lane, the tail and EndMark by its last lane: once each, through the complete table.
+// Counters: every lane keeps CountKernel's registers and flushes them into its warp's row of u32 in shared memory (shared
+// atomics, one flush per 120 chunks).  A warp walks at most 80 GB / 4 224 warps (19 MB) of an H100's memory, 15 per byte
+// at most, well inside 32 bits.  At the end every CTA adds its warps' rows into the caller's u64 counters with one 64-bit
+// atomic per regexp.  With more regexps than kCountRowsMax the rows do not fit; flushes then go to the u64 counters.
+// The plain walk locates: it is the one AUTO runs for pire_gpu_run_string on every automaton (ResolveVariant, non-uniform),
+// and the counting walk is plain as well, so the two phases share their code shape.
+template <int kWords, bool kAlways>
+__global__ void __launch_bounds__(kBlock, kStringBlocksPerSM) CountStringKernel(const __grid_constant__ ScanArgs a)
+{
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    uint8_t* const smem = pire_b200_smem;
+    SharedView sv = CarveShared(smem, a.hot);
+    StageTables(a, sv, a.hot8, a.hot);
+    // behind the marks: the hot states' packed increments (zeros for the sink), then every warp's row of counters
+    uint64_t* const hot_w = reinterpret_cast<uint64_t*>(sv.stage + kSplitMarkBytes);
+    uint32_t* const rows = reinterpret_cast<uint32_t*>(hot_w + (size_t) (a.hot + 1) * kWords);
+    if (kWords > 0)
+        for (uint32_t i = threadIdx.x; i < (a.hot + 1) * kWords; i += blockDim.x)
+            hot_w[i] = i < a.hot * kWords ? a.weights[i] : 0;
+    if (a.count_rows)
+        for (uint32_t i = threadIdx.x; i < kWarpsPerBlock * a.regexps; i += blockDim.x)
+            rows[i] = 0;
+    __syncthreads();
+
+    Tables t;
+    t.hot = sv.hot;
+    t.base = SmemAddr(sv.hot);
+    t.cls = sv.cls;
+    t.full = a.full;
+    t.H = a.hot;
+    t.letters = a.letters;
+    t.wide = a.wide;
+    t.m0 = a.exit_bitmap0;
+
+    // the true start, as in ScanStringKernel (*a.start_idx may be the output word: written only after the last grid.sync())
+    uint32_t start = a.start;
+    bool valid = true;
+    if (a.start_idx)
+        StartFrom(a, t, *a.start_idx, start, valid);
+    const bool skip = !valid || (start < t.H && sv.noexit[start] != 0);       // multi.h:955-958: no byte leaves it
+
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t warp = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
+    const uint32_t warps = gridDim.x * kWarpsPerBlock;
+    uint8_t* const marks = sv.stage + (threadIdx.x >> 5) * (32 * kSplitMarks) + lane;
+    const uintptr_t buf_lo = reinterpret_cast<uintptr_t>(a.corpus);
+    const uintptr_t buf_hi = buf_lo + a.fixed_len;
+    const uint8_t* const end = a.corpus + a.fixed_len;
+
+    // phase 1, locate: the head by the grid's first warp, then the pieces (ScanStringKernel)
+    LaneState s;
+    SetFull(t, s, start);
+    if (warp == 0 && !skip) {
+        const uint8_t* p = a.corpus;
+        const uint32_t mis = (uint32_t) (buf_lo & 15);
+        if (p < end && mis != 0) {
+            const uint64_t room = (uint64_t) (end - p);
+            const uint32_t nhead = room < 16 - mis ? (uint32_t) room : 16 - mis;
+            EdgeFast<false>(t, s, EdgeBytes(LoadChunk16(p - mis, buf_lo, buf_hi), mis).Words(), nhead);
+            p += nhead;
+        }
+        if ((reinterpret_cast<uintptr_t>(p) & 16) && end - p >= 16)
+            Chunk16<false>(t, s, LoadEdge16(p));
+    }
+    const uint8_t* const body = StringBody(a.corpus, end);
+    const uint32_t blocks_total = (reinterpret_cast<uintptr_t>(body) & 31) ? 0u : (uint32_t) ((end - body) >> 5);
+    const uint32_t lanes = gridDim.x * kBlock;
+    const uint32_t me = blockIdx.x * kBlock + threadIdx.x;
+    const uint32_t base = blocks_total / lanes, rem = blocks_total % lanes;
+    const uint32_t my_blocks = base + (me < rem ? 1u : 0u);
+    const uint64_t my_first = (uint64_t) me * base + (me < rem ? me : rem);
+    const uint32_t trips = base + (rem ? 1u : 0u);
+    const uint32_t per_mark = (trips + kSplitMarks - 1) / kSplitMarks;
+    const uint8_t* const piece = body + 32 * my_first;
+    const uint32_t first_start = __shfl_sync(0xffffffffu, FullState(t, s), 0);
+
+    uint32_t start_full = me == 0 ? first_start : 0u;
+    uint32_t end_full = start_full;
+    if (!skip) {
+        SetFull(t, s, start_full);
+        WalkPiece<false>(t, s, piece, my_blocks, trips, per_mark, marks, 0);
+        end_full = FullState(t, s);
+
+        uint4 head0 = make_uint4(0, 0, 0, 0), head1 = head0;
+        bool head_fresh = my_blocks != 0;
+        if (head_fresh)
+            LoadStream32P(piece, head0, head1);
+        PIRE_B200_STITCH_GRID(false);
+    } else {
+        grid.sync();
+    }
+    if (!valid) {
+        // a start outside the scanner reads no table and counts nothing: match 0, state 0xFFFFFFFF
+        if (me == lanes - 1) {
+            if (a.match_bits)
+                a.match_bits[0] = 0;
+            if (a.state_idx)
+                a.state_idx[0] = 0xFFFFFFFFu;
+        }
+        return;
+    }
+    if (skip)
+        start_full = start;  // a NoExit start: every piece starts (and stays) there, and each of its steps is counted
+
+    // phase 2, count
+    Counter<kWords, WarpRow> c;
+    c.Reset(a, hot_w, WarpRow{a.count_rows ? rows + (threadIdx.x >> 5) * a.regexps : nullptr, a.counts64});
+    if (me == 0) {
+        // Initialize() ends in TakeAction (half_final.h:136-141); a resumed run counted its start in the previous call.
+        // `start` is the state after BeginMark when it was asked for.
+        if (!a.start_idx)
+            c.Step(a, t.H, a.initial);
+        if (a.with_begin)
+            c.Step(a, t.H, start);
+        c.EndGroup(a.regexps);
+        uint32_t full = start;
+        for (const uint8_t* p = a.corpus; p < body; ++p) {
+            full = SlowStep(t, full, *p);
+            c.Step(a, t.H, full);
+            c.EndGroup(a.regexps);
+        }
+    }
+    SetFull(t, s, start_full);
+    if (my_blocks != 0) {
+        const uint32_t len = 32u * my_blocks;
+        uint4 a0, a1, b0, b1;
+        LoadStream32(piece, a0, a1);
+        for (uint32_t off = 0;;) {
+            off += 32;
+            const bool more_b = off < len;
+            if (more_b)
+                LoadStream32(piece + off, b0, b1);
+            CountChunk16<kWords, kAlways>(a, t, s, a0, c);
+            CountChunk16<kWords, kAlways>(a, t, s, a1, c);
+            if (!more_b)
+                break;
+            off += 32;
+            const bool more_a = off < len;
+            if (more_a)
+                LoadStream32(piece + off, a0, a1);
+            CountChunk16<kWords, kAlways>(a, t, s, b0, c);
+            CountChunk16<kWords, kAlways>(a, t, s, b1, c);
+            if (!more_a)
+                break;
+        }
+    }
+    if (me == lanes - 1) {
+        // the tail from the last piece's end, EndMark, and the results (those of ScanStringKernel)
+        uint32_t last = FullState(t, s);
+        for (const uint8_t* p = body + 32 * (size_t) blocks_total; p < end; ++p) {
+            last = SlowStep(t, last, *p);
+            c.Step(a, t.H, last);
+            c.EndGroup(a.regexps);
+        }
+        if (a.through_end) {
+            c.Step(a, t.H, FullNext(t, last, a.end_class));          // Step(EndMark)
+            c.EndGroup(a.regexps);
+        }
+        const DeviceFin f = a.fin[last];
+        if (a.match_bits)
+            a.match_bits[0] = f.result >> 31;
+        if (a.state_idx)
+            a.state_idx[0] = f.result & 0x7fffffffu;
+    }
+    c.Finish(a.regexps);
+    if (!a.count_rows)
+        return;
+    __syncthreads();
+    for (uint32_t id = threadIdx.x; id < a.regexps; id += blockDim.x) {
+        unsigned long long sum = 0;
+        for (uint32_t w = 0; w < kWarpsPerBlock; ++w)
+            sum += rows[w * a.regexps + id];
+        if (sum)
+            atomicAdd(a.counts64 + id, sum);
     }
 }
 
@@ -3535,18 +3754,15 @@ cudaError_t LaunchSplit(const ScanArgs& a, int variant, int device, cudaStream_t
     return err;
 }
 
-// One string (a.corpus, a.fixed_len bytes) over the persistent grid (ScanStringKernel).  The grid is the occupancy
+// One string (a.corpus, a.fixed_len bytes) over the persistent grid (ScanStringKernel, CountStringKernel).  The grid is the occupancy
 // query's, cut to one CTA per kBlock * kStringMinBlocks blocks of body so that pieces do not get short; every length,
 // down to 0, goes through the kernel.  a.string_ends / a.string_rounds are filled in here from per-call scratch.
-cudaError_t LaunchString(const ScanArgs& a, int variant, int device, cudaStream_t stream)
+static cudaError_t LaunchStringGrid(const void* fn, const ScanArgs& a, size_t shared, int device, cudaStream_t stream)
 {
     static const uint32_t min_blocks = [] {
         const char* env = getenv("PIRE_B200_STRING_MIN_BLOCKS");  // experiments: 32-byte blocks per lane before CTAs are cut
         return env && atoi(env) >= 1 ? (uint32_t) atoi(env) : kStringMinBlocks;
     }();
-    const void* fn = variant == kVariantPlain ? reinterpret_cast<const void*>(&ScanStringKernel<false>)
-                                              : reinterpret_cast<const void*>(&ScanStringKernel<true>);
-    const size_t shared = ScanSharedBytes(a.hot, 0) + kSplitMarkBytes;
     int optin = 0, sms = 0, per_sm = 0;
     cudaError_t err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
     if (err == cudaSuccess)
@@ -3580,6 +3796,29 @@ cudaError_t LaunchString(const ScanArgs& a, int variant, int device, cudaStream_
         g_launches.fetch_add(1, std::memory_order_relaxed);
     cudaFreeAsync(scratch, stream);
     return err;
+}
+
+cudaError_t LaunchString(const ScanArgs& a, int variant, int device, cudaStream_t stream)
+{
+    const void* fn = variant == kVariantPlain ? reinterpret_cast<const void*>(&ScanStringKernel<false>)
+                                              : reinterpret_cast<const void*>(&ScanStringKernel<true>);
+    return LaunchStringGrid(fn, a, ScanSharedBytes(a.hot, 0) + kSplitMarkBytes, device, stream);
+}
+
+// Behind the tables and the marks: the hot states' packed increments, then (a.count_rows) one row of u32 per warp.
+cudaError_t LaunchCountString(const ScanArgs& a, int device, cudaStream_t stream)
+{
+    const void* fn = nullptr;
+    switch (a.count_words * 2 + (a.count_always ? 1 : 0)) {
+    case 2: fn = reinterpret_cast<const void*>(&CountStringKernel<1, false>); break;
+    case 3: fn = reinterpret_cast<const void*>(&CountStringKernel<1, true>); break;
+    case 4: fn = reinterpret_cast<const void*>(&CountStringKernel<2, false>); break;
+    case 5: fn = reinterpret_cast<const void*>(&CountStringKernel<2, true>); break;
+    default: fn = reinterpret_cast<const void*>(&CountStringKernel<0, false>); break;
+    }
+    const size_t shared = ScanSharedBytes(a.hot, 0) + kSplitMarkBytes + (size_t) (a.hot + 1) * a.count_words * 8
+                          + (a.count_rows ? (size_t) kWarpsPerBlock * a.regexps * 4 : 0);
+    return LaunchStringGrid(fn, a, shared, device, stream);
 }
 
 cudaError_t LaunchPrefix(const ScanArgs& a, bool shortest, bool reverse, int device, cudaStream_t stream)

@@ -78,6 +78,9 @@ struct ScanArgs {
     // mapped through new_of_old, BeginMark stepped when with_begin; one at or above `states` reports (0, 0, 0xFFFFFFFF).
     // starts may be state_idx: every kernel reads string i's start before it writes string i's state
     const uint32_t* starts;      // n words, or null: every string starts from `start`
+    // counting one string over the grid (pire_gpu_count_string): the counts are added to counts64 (max(1, regexps) words)
+    unsigned long long* counts64;
+    uint32_t count_rows;         // 1: every warp sums into a row of u32 in shared memory first; 0: straight into counts64
 };
 
 struct LaunchPlan {
@@ -112,6 +115,11 @@ cudaError_t LaunchSplit(const ScanArgs& a, int variant, int device, cudaStream_t
 // one string (a.corpus, a.fixed_len bytes) over the whole grid, cooperatively launched; a.with_begin / a.begin_class
 // step BeginMark from *a.start_idx when that is given
 cudaError_t LaunchString(const ScanArgs& a, int variant, int device, cudaStream_t stream);
+// HalfFinalScanner counts of one string over the whole grid (CountStringKernel): LaunchString's grid and pieces, the
+// counting fields of LaunchCount, a.counts64 added to; a.start_idx / a.with_begin as in LaunchString
+cudaError_t LaunchCountString(const ScanArgs& a, int device, cudaStream_t stream);
+// the largest max(1, regexps) for which LaunchCountString keeps a row of counters per warp in shared memory
+constexpr uint32_t kCountRowsMax = 256;
 cudaError_t LaunchVisitCount(const ScanArgs& a, cudaStream_t stream);
 // prefix (left to right) or suffix (right to left) scan; a.with_begin/begin_class name the mark stepped first,
 // a.through_end/end_class the mark stepped last

@@ -419,6 +419,90 @@ class StringRunner:
         return self.Sc.AcceptedRegexps(self.State())
 
 
+class StringCounter:
+    """A Pire::HalfFinalScanner run over ONE string resident in HBM, counted by the whole GPU (pire_gpu_count_string):
+    ``Result(r)`` is the number of positions where a match of regexp r ends.  ``Run(text)`` may be called many times:
+    the texts are counted as one string, the state carried from call to call in a device word and the counts added to
+    a zeroed device tensor of u64 (``Counts()``), so chained calls do not synchronise.  ``state`` = a StateIndex to
+    resume from (not counted again: the run that reached it counted it), None = Initialize() (counted).  Every
+    ``Run()`` launches at once on the current stream; ``Begin()`` is folded into the first launch, ``End()`` is a launch
+    of its own.  Results (``Result()``, ``AcceptedRegexps()``, ``Final()``, ``State()``) synchronise."""
+
+    def __init__(self, sc, state=None):
+        self.Sc = sc
+        self._start = None if state is None else int(state)
+        self._words = None         # device: [StateIndex, match word]
+        self._counts = None        # device: max(1, regexps) u64
+        self._begin = False
+        self._ran = False
+
+    def Begin(self):
+        if self._ran:
+            raise ValueError("Begin() must precede Run()")
+        self._begin = True
+        return self
+
+    def Run(self, text):
+        torch = _torch()
+        if text.dtype != torch.uint8 or not text.is_cuda or not text.is_contiguous() or text.device.index != self.Sc.device:
+            raise ValueError("text must be a contiguous uint8 CUDA tensor on the scanner's device")
+        self._launch(text, 0)
+        return self
+
+    def End(self):
+        self._launch(None, N.RUN_END)
+        return self
+
+    def _launch(self, text, flags):
+        if self._begin:
+            flags |= N.RUN_BEGIN
+            self._begin = False
+        start = stream = words = counts = None
+        if self.Sc.device >= 0:
+            torch = _torch()
+            dev = torch.device("cuda", self.Sc.device)
+            if self._words is None:
+                self._words = torch.empty(2, dtype=torch.int32, device=dev)
+                self._counts = torch.zeros(max(1, self.Sc.RegexpsCount()), dtype=torch.int64, device=dev)
+                if self._start is not None:
+                    word = self._start & 0xFFFFFFFF
+                    self._words[0] = word - (1 << 32) if word >= (1 << 31) else word
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            if self._ran or self._start is not None:
+                start = self._words.data_ptr()
+            words, counts = self._words.data_ptr(), self._counts.data_ptr()
+        N.check(N.lib.pire_gpu_count_string(self.Sc._h, None if text is None else text.data_ptr(), 0 if text is None else text.numel(),
+                                            flags, start, counts, None if words is None else words + 4, words, stream),
+                "pire_gpu_count_string")
+        self._ran = True
+
+    def _results(self):
+        if not self._ran:
+            self._launch(None, 0)          # nothing run yet: the start state itself (after Begin() if it was asked for)
+        return self._words.cpu().numpy().view(np.uint32)
+
+    def Counts(self):
+        """The device tensor of counters (int64 holding u64), one per regexp; does not synchronise."""
+        if not self._ran:
+            self._launch(None, 0)
+        return self._counts
+
+    def Result(self, regexp_id):
+        """State::Result(regexp_id) (half_final.h:88-90)."""
+        return int(self.Counts()[regexp_id].item())
+
+    def AcceptedRegexps(self):
+        """HalfFinalScanner::AcceptedRegexps (half_final.h:130-133): regexps with a non-zero counter."""
+        return [int(r) for r in np.nonzero(self.Counts().cpu().numpy())[0]]
+
+    def State(self):
+        """StateIndex() of the state reached (reference numbering); 0xFFFFFFFF for a start outside the scanner."""
+        return int(self._results()[0])
+
+    def Final(self):
+        return bool(self._results()[1] & 1)
+
+
 def Runner(sc, states=None):
     """Pire::Runner(sc) (run.h:388-389); with ``states`` Pire::Runner(sc, st) (run.h:391-392) for every string."""
     return RunHelper(sc, states)
