@@ -413,18 +413,7 @@ static int PrefixOrSuffix(const pire_gpu_scanner* sc, const uint8_t* d_corpus, c
     a.end_class = reverse ? sc->tab.begin_class : sc->tab.end_class;
     a.prefix_len = d_len;
     a.first_final_hot = sc->tab.first_final_hot;
-    a.uniform = (!reverse && IsUniform(d_corpus, d_offsets, fixed_len) && !getenv("PIRE_B200_NO_UNIFORM_BODY")) ? 1 : 0;
-    if (a.uniform) {
-        // the uniform prefix kernel walks plain: with the exit filter of hot id 0 its step is five ALU-pipe instructions
-        // (PRMT, SHF, 2 x LOP3, VIMNMX), about twice the plain step's;
-        // PIRE_B200_PREFIX_PRED=1 selects the filtered walk for experiments
-        static const int forced = [] {
-            const char* env = getenv("PIRE_B200_PREFIX_PRED");
-            return env ? atoi(env) : 0;
-        }();
-        const bool pred = forced != 0;
-        a.uniform = pred ? 2 : 1;
-    }
+    a.uniform = (!reverse && IsUniform(d_corpus, d_offsets, fixed_len)) ? 1 : 0;
     CUDA_TRY(LaunchPrefix(a, shortest != 0, reverse, sc->device, static_cast<cudaStream_t>(stream)));
     return PIRE_GPU_OK;
 }
@@ -473,7 +462,7 @@ int pire_gpu_count_batch(const pire_gpu_scanner* sc, const uint8_t* d_corpus, co
     a.weights = sc->dev.weights;
     a.count_words = sc->count_mode == 1 ? 0 : sc->tab.count_words;
     a.count_always = (sc->count_mode == 3 || (sc->count_mode == 0 && sc->final_share > 0.025)) ? 1 : 0;
-    a.uniform = (IsUniform(d_corpus, d_offsets, fixed_len) && !getenv("PIRE_B200_NO_UNIFORM_BODY")) ? 1 : 0;
+    a.uniform = IsUniform(d_corpus, d_offsets, fixed_len) ? 1 : 0;
     CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t) n * a.regexps * 4, st));
     CUDA_TRY(LaunchCount(a, sc->device, st));
     return PIRE_GPU_OK;
@@ -592,11 +581,7 @@ static int RunCsr(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uin
     a.state_idx = d_state_idx;
     unsigned int* counter = nullptr;
     cudaError_t ce = cudaSuccess;
-    static const bool split_long = [] {
-        const char* env = getenv("PIRE_B200_SPLIT");              // experiments: 0 = long strings stay one per lane
-        return !(env && env[0] == '0');
-    }();
-    const bool split = d_order && split_long && !(flags & PIRE_GPU_RUN_LINES);
+    const bool split = d_order && !(flags & PIRE_GPU_RUN_LINES);
     if (d_order) {
         // length-binned: units are claimed longest-first, match bits are OR-ed into a zeroed bitmap; three words:
         // the generic kernel's unit counter, the split kernel's string counter, the number of strings it owns
@@ -616,11 +601,7 @@ static int RunCsr(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uin
         SetStarts(sc, &a, d_start, flags);
     if (split && ce == cudaSuccess)
         ce = LaunchSplit(a, (int) variant, sc->device, st);       // the long strings, one per warp; the rest below
-    static const bool lines_kernel = [] {
-        const char* env = getenv("PIRE_B200_LINES_KERNEL");       // experiments: 0 = lines go through the generic kernel
-        return !(env && env[0] == '0');
-    }();
-    if ((flags & PIRE_GPU_RUN_LINES) && !d_order && lines_kernel) {
+    if ((flags & PIRE_GPU_RUN_LINES) && !d_order) {
         // lines of text: lanes pull lines dynamically and OR their match bits into a zeroed bitmap
         if (d_match_bits)
             ce = cudaMemsetAsync(d_match_bits, 0, (size_t) ((n + 31) / 32) * 4, st);

@@ -22,7 +22,7 @@
 //   * LOOK variant (the glued benchmark scan): the filter looks one byte further -- a resting
 //     lane reads the table only if this byte and the next both pass -- in 5.5 instructions per
 //     byte (LookProbe / LookStep), two strings per lane (ScanUniformLookRingKernel, fed from a per-lane cp.async ring
-//     with two blocks of each string in flight; ScanUniformLook2Kernel, fed from registers).  The LOOK_RING1 variant walks
+//     with two blocks of each string in flight).  The LOOK_RING1 variant walks
 //     one string per lane from such a ring, 32 warps per SM (ScanUniformLookRing1Kernel).
 //   * Input bytes: each lane streams its own string: 32-byte read-only loads (two
 //     LDG.128 of one sector, the second an L1 hit), one ahead in a register ping-pong (uniform kernels,
@@ -681,9 +681,7 @@ __device__ __forceinline__ void LookBlock32(const Tables& t, uint32_t& g, uint32
 // Register budget.  The register file is split between the four warp schedulers (16 K registers each), so a
 // CTA's warps should be a multiple of four: 512 threads x 3 CTAs leaves 40 registers per thread (12 warps x 1280
 // per scheduler), 384 threads x 3 CTAs or 640 threads x 2 CTAs leave 48 (9 / 10 warps x 1536).  The kernel is short
-// of independent chains, so the ten-warp shape is the default; both instantiations
-// exist (PIRE_B200_LOOK_REGS=40|48, PIRE_B200_LOOK_BLOCK=<threads> for experiments).
-constexpr int kLookBlock40 = 512;
+// of independent chains, so it runs the ten-warp shape at 48 registers.
 constexpr int kLookBlock48 = 640;
 
 template <bool k64, int kRegs, bool kClean, bool kStarts>
@@ -765,7 +763,7 @@ __global__ void __maxnreg__(kRegs) ScanUniformLookKernel(const __grid_constant__
 // The one-string look-ahead kernel waits mostly on the LOP3 that needs the previous step's LDS, and more warps per SM
 // run it faster -- it is short of independent chains, and registers (48 per thread) cap the warps.  Here every lane walks TWO strings (units 2p and 2p+1 of the
 // batch) step by step in turn: the second string's step fills the latency of the first one's table read, and the
-// block bookkeeping is shared.  32 data registers (two ping-pong sets of 32 bytes), __maxnreg__ chosen by the launch plan.
+// block bookkeeping is shared.
 template <bool kClean>
 __device__ __forceinline__ void LookWord2(uint32_t& ga, uint32_t wa, uint32_t bba0, uint32_t paa0, uint32_t pana, uint32_t& gb, uint32_t wb,
                                           uint32_t bbb0, uint32_t pab0, uint32_t panb, uint32_t base, const LookFilter& f)
@@ -787,9 +785,8 @@ __device__ __forceinline__ void LookWord2(uint32_t& ga, uint32_t wa, uint32_t bb
     LookStep<kClean>(gb, bbb3, pab3, panb);
 }
 
-// `late(ga, gb, nexta, nextb)` fetches the first words of the blocks that follow, after the walk of the block's first 28
-// bytes (see LookBlock32): from registers loaded a block ahead (ScanUniformLook2Kernel) or from the ring in shared memory
-// (ScanUniformLookRingKernel).
+// `late(ga, gb, latea, lateb)` fetches the first words of the blocks that follow, after the walk of the block's first 28
+// bytes (see LookBlock32), from the ring in shared memory (ScanUniformLookRingKernel).
 template <bool kClean, typename Late>
 __device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uint32_t& preva, const uint4& a0, const uint4& a1,
                                               uint32_t& gb, uint32_t& prevb, const uint4& b0, const uint4& b1, bool more,
@@ -837,108 +834,11 @@ __device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uin
     }
 }
 
-// The next words are in registers, loaded a block ahead: they are made to depend on the walk itself -- plus g times a
-// kernel argument that is always zero -- so that their probes stay behind it.
-template <bool kClean>
-__device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uint32_t& preva, const uint4& a0, const uint4& a1, uint32_t nexta,
-                                              uint32_t& gb, uint32_t& prevb, const uint4& b0, const uint4& b1, uint32_t nextb, bool more,
-                                              const LookFilter& f, uint32_t opaque_zero, const ScanArgs* args)
-{
-    LookBlock32x2<kClean>(t, ga, preva, a0, a1, gb, prevb, b0, b1, more, f,
-                          [=](uint32_t ga, uint32_t gb, uint32_t& latea, uint32_t& lateb) {
-                              latea = nexta + ga * opaque_zero;
-                              lateb = nextb + gb * opaque_zero;
-                          },
-                          args);
-}
-
-template <int kRegs>
-__global__ void __maxnreg__(kRegs) ScanUniformLook2Kernel(const __grid_constant__ ScanArgs a)
-{
-    uint8_t* const smem = pire_b200_smem;
-    SharedView sv = CarveShared(smem, a.hot);
-    StageTables(a, sv, a.hot8, a.hot);
-
-    Tables t;
-    t.hot = sv.hot;
-    t.base = SmemWindowBase();
-    t.cls = sv.cls;
-    t.full = a.full;
-    t.H = a.hot;
-    t.letters = a.letters;
-    t.wide = a.wide;
-    t.m0 = a.look_bitmap;
-    LookFilter f;
-    f.lo = a.look_bitmap;
-    f.hi = 0;
-    f.zero = a.opaque_zero;
-    f.rev = __brev(f.lo);
-
-    const uint32_t units = (uint32_t) ((a.n + 31) / 32);
-    const uint32_t pairs = (units + 1) / 2;
-    const uint32_t warps_per_block = blockDim.x >> 5;
-    const uint32_t warps = gridDim.x * warps_per_block;
-    const uint32_t len = (uint32_t) a.fixed_len;
-    const uint32_t blocks = len >> 5;
-
-    for (uint32_t pair = blockIdx.x * warps_per_block + (threadIdx.x >> 5); pair < pairs; pair += warps) {
-        const bool second = 2 * pair + 1 < units;          // the last pair of an odd batch walks its first unit twice
-        uint32_t ga, preva, gb, prevb;
-        {
-            const uint64_t ia = (uint64_t) pair * 64 + (threadIdx.x & 31);
-            const uint64_t ib = ia + (second ? 32 : 0);
-            const uint8_t* pa = a.corpus + (ia < a.n ? ia : a.n - 1) * (uint64_t) len;
-            const uint8_t* pb = a.corpus + (ib < a.n ? ib : a.n - 1) * (uint64_t) len;
-            preva = prevb = a.start;
-            ga = gb = a.start < t.H ? a.start : t.H;
-            if (blocks != 0) {
-                uint4 a0, a1, b0, b1, c0, c1, d0, d1;         // a/c: the first string's ping-pong sets, b/d: the second's
-                LoadStream32(pa, a0, a1);
-                LoadStream32(pb, b0, b1);
-                for (uint32_t left = blocks;;) {
-                    const bool more_c = left > 1;
-                    pa += 32;
-                    pb += 32;
-                    if (more_c) {
-                        LoadStream32(pa, c0, c1);
-                        LoadStream32(pb, d0, d1);
-                    }
-                    __syncwarp();          // scheduling fence: the loads stay up here (see ScanUniformLookKernel)
-                    LookBlock32x2<true>(t, ga, preva, a0, a1, c0.x, gb, prevb, b0, b1, d0.x, more_c, f, a.opaque_zero, &a);
-                    if (!more_c)
-                        break;
-                    const bool more_a = left > 2;
-                    pa += 32;
-                    pb += 32;
-                    if (more_a) {
-                        LoadStream32(pa, a0, a1);
-                        LoadStream32(pb, b0, b1);
-                    }
-                    __syncwarp();
-                    LookBlock32x2<true>(t, ga, preva, c0, c1, a0.x, gb, prevb, d0, d1, b0.x, more_a, f, a.opaque_zero, &a);
-                    left -= 2;
-                    if (!more_a || __all_sync(0xffffffffu, (sv.noexit[ga] & sv.noexit[gb]) != 0))
-                        break;
-                }
-            }
-        }
-        const uint64_t ia = (uint64_t) pair * 64 + (threadIdx.x & 31);
-        LaneState s;
-        s.g = t.H;
-        s.cold = ga == t.H ? preva : ga;
-        Report(a, t, s, 2 * (uint64_t) pair, ia, ia < a.n);
-        if (second) {
-            s.cold = gb == t.H ? prevb : gb;
-            Report(a, t, s, 2 * (uint64_t) pair + 1, ia + 32, ia + 32 < a.n);
-        }
-    }
-}
-
 // ---------------------------------------------------------------- LOOK variant, two strings per lane, fed from a ring
 //
-// ScanUniformLook2Kernel keeps one 32-byte block of each string in flight, and that load shape alone moves about half of
-// what HBM can deliver: the scan is bound by its loads, not by the walk.  More blocks in flight per string would take
-// registers the kernel does not have, so here each lane copies its blocks with cp.async (LDGSTS) into a private ring in
+// Two strings per lane fed from registers, one 32-byte block of each string in flight (a kernel since removed), moved
+// about half of what HBM can deliver: the scan is bound by its loads, not by the walk.  More blocks in flight per string
+// would take registers such a kernel does not have, so here each lane copies its blocks with cp.async (LDGSTS) into a private ring in
 // shared memory, three slots per string, and reads a block into registers (two LDS.128 per string) only when it walks
 // it: two blocks of each string are on their way while one is walked.  Same walk, same pairs of units, same NoExit exit
 // every 64 bytes; one CTA of 24 warps per SM.  The shape is the fastest of the ring shapes tools/microbench.cu measures
@@ -2020,7 +1920,7 @@ __global__ void __launch_bounds__(kBlock, kMinBlocksPerSM) ScanLinesKernel(const
 // ---------------------------------------------------------------- lines of text, in stream
 //
 // The lines of a newline-delimited text lie back to back, so they can be scanned where they are: the text is cut
-// into segments of a.text_segment bytes on 32-byte boundaries of the address space, lane j of a warp walks segment
+// into segments of about kTextSegment bytes on 32-byte boundaries of the address space, lane j of a warp walks segment
 // 32 * unit + j like the uniform kernel walks a string (32-byte loads, one block ahead in registers, every lane busy in
 // every step), and owns the lines that START inside its segment -- it runs past the segment's end until the last of
 // them is finished.  What makes this cheap:
@@ -2217,13 +2117,10 @@ __global__ void __launch_bounds__(kBlock, kTextBlocksPerSM) ScanTextKernel(const
     const uint64_t warps = (uint64_t) gridDim.x * kWarpsPerBlock;
     // Segment size: about kTextSegment bytes, chosen so that the units (32 segments) come out as a whole number of
     // rounds over the grid's warps -- with a couple of units per warp, one unit more or less is a third of the run time.
-    uint64_t seg = a.text_segment;
-    if (seg == 0) {
-        const uint64_t lanes = 32 * warps;
-        const uint64_t rounds = (total + 64 + lanes * kTextSegment - 1) / (lanes * kTextSegment);
-        seg = ((total + 64 + lanes * rounds - 1) / (lanes * rounds) + 31) / 32 * 32;
-        seg = seg < 64 ? 64 : seg;
-    }
+    const uint64_t lanes = 32 * warps;
+    const uint64_t rounds = (total + 64 + lanes * kTextSegment - 1) / (lanes * kTextSegment);
+    uint64_t seg = ((total + 64 + lanes * rounds - 1) / (lanes * rounds) + 31) / 32 * 32;
+    seg = seg < 64 ? 64 : seg;
     const uint64_t segments = (total + mis0) / seg + 1;
     const uint64_t units = (segments + 31) / 32;
 
@@ -2490,7 +2387,7 @@ __device__ __forceinline__ void PrefixCheck(const ScanArgs& a, uint32_t H, const
         l.stop = true;
 }
 
-template <bool kShortest, bool kReverse, bool kPred = false, bool kIdp = false>
+template <bool kShortest, bool kReverse>
 __device__ __forceinline__ void PrefixChunk16(const ScanArgs& a, const Tables& t, const uint8_t* hot_flags, LaneState& s, uint4 v,
                                               PrefixLane& l)
 {
@@ -2502,7 +2399,7 @@ __device__ __forceinline__ void PrefixChunk16(const ScanArgs& a, const Tables& t
         const uint32_t word = at == 0 ? v.x : at == 1 ? v.y : at == 2 ? v.z : v.w;
 #pragma unroll
         for (int b = 0; b < 4; ++b) {
-            FastStep<kPred, kIdp>(t, g, word, 0x5540 + (kReverse ? 3 - b : b));
+            FastStep<false, false>(t, g, word, 0x5540 + (kReverse ? 3 - b : b));
             top = max(top, g);
             if (!kShortest)
                 low = min(low, g);
@@ -2535,7 +2432,7 @@ __device__ __forceinline__ void PrefixChunk16(const ScanArgs& a, const Tables& t
             const uint32_t word = at == 0 ? v.x : at == 1 ? v.y : at == 2 ? v.z : v.w;
 #pragma unroll
             for (int b = 0; b < 4; ++b) {
-                FastStep<kPred, kIdp>(t, h, word, 0x5540 + (kReverse ? 3 - b : b));
+                FastStep<false, false>(t, h, word, 0x5540 + (kReverse ? 3 - b : b));
                 const bool final = h >= a.first_final_hot;
                 if (kShortest)
                     mark = final && mark == 0 ? (uint32_t) (4 * w + b + 1) : mark;
@@ -2785,11 +2682,11 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) PrefixKernel(cons
 }
 
 // Forward prefix scans of a fixed-length, 32-byte aligned batch (the BASELINE configs' shape) in a kernel of their own:
-// no edge bytes and no staging ring, so three CTAs (or two of twenty warps) fit an SM instead of the generic kernel's two
-// of sixteen, and the walk can use the exit filter of hot id 0 (kPred): a lane resting there on a byte that cannot leave
-// keeps g = 0, which is all the running maximum needs.  (The look-ahead filter does not carry over: it skips the one-step
-// states behind an exit byte, and a prefix scan must see them if they are final.)
-template <bool kShortest, bool kPred, bool kIdp>
+// no edge bytes and no staging ring, so two CTAs of twenty warps fit an SM instead of the generic kernel's two of
+// sixteen.  The walk is plain: with the exit filter of hot id 0 its step is five ALU-pipe instructions (PRMT, SHF,
+// 2 x LOP3, VIMNMX), about twice the plain step's.  (The look-ahead filter does not carry over at all: it skips the
+// one-step states behind an exit byte, and a prefix scan must see them if they are final.)
+template <bool kShortest>
 __global__ void __maxnreg__(48) PrefixUniformKernel(const __grid_constant__ ScanArgs a)
 {
     uint8_t* const smem = pire_b200_smem;
@@ -2808,7 +2705,6 @@ __global__ void __maxnreg__(48) PrefixUniformKernel(const __grid_constant__ Scan
     t.H = a.hot;
     t.letters = a.letters;
     t.wide = a.wide;
-    t.m0 = a.exit_bitmap0;
 
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t warps_per_block = blockDim.x >> 5;
@@ -2845,9 +2741,9 @@ __global__ void __maxnreg__(48) PrefixUniformKernel(const __grid_constant__ Scan
                 if (more_b)
                     LoadStream32(src + off, b0, b1);
                 if (!l.stop)
-                    PrefixChunk16<kShortest, false, kPred, kIdp>(a, t, hot_flags, s, a0, l);
+                    PrefixChunk16<kShortest, false>(a, t, hot_flags, s, a0, l);
                 if (!l.stop)
-                    PrefixChunk16<kShortest, false, kPred, kIdp>(a, t, hot_flags, s, a1, l);
+                    PrefixChunk16<kShortest, false>(a, t, hot_flags, s, a1, l);
                 if (!more_b)
                     break;
                 off += 32;
@@ -2855,9 +2751,9 @@ __global__ void __maxnreg__(48) PrefixUniformKernel(const __grid_constant__ Scan
                 if (more_a)
                     LoadStream32(src + off, a0, a1);
                 if (!l.stop)
-                    PrefixChunk16<kShortest, false, kPred, kIdp>(a, t, hot_flags, s, b0, l);
+                    PrefixChunk16<kShortest, false>(a, t, hot_flags, s, b0, l);
                 if (!l.stop)
-                    PrefixChunk16<kShortest, false, kPred, kIdp>(a, t, hot_flags, s, b1, l);
+                    PrefixChunk16<kShortest, false>(a, t, hot_flags, s, b1, l);
                 // a dead state only leads to dead states: stop the lane once it is noticed (every 64 bytes)
                 if (!l.stop) {
                     const uint32_t at = FullState(t, s);
@@ -3509,113 +3405,53 @@ __global__ void __launch_bounds__(256) SynthMixedFillKernel(uint64_t seed, uint3
     }
 }
 
-template <bool kPred, bool kStarts = false>
-const void* UniformKernelPtr() { return reinterpret_cast<const void*>(&ScanUniformKernel<kPred, kStarts>); }
-template <int kMode, bool kStarts = false>
-const void* GenericKernelPtr() { return reinterpret_cast<const void*>(&ScanGenericKernel<kMode, kStarts>); }
-
-int LookRegs()
+// The walk a variant takes in the generic (CSR) kernel, its kMode: 0 plain (PLAIN, PRIV), 1 exit filter (PRED), 2 exit
+// filter with one byte of look-ahead (the LOOK variants).  The lines kernels walk with the exit filter for 1 and 2.
+int WalkMode(int variant)
 {
-    static const int regs = [] {
-        const char* env = getenv("PIRE_B200_LOOK_REGS");
-        return env && atoi(env) == 40 ? 40 : 48;
-    }();
-    return regs;
-}
-
-// PIRE_B200_LOOK_CLEAN=0 restores the two-LOP3 step of the look-ahead kernel (see LookProbe) for comparison.
-bool LookClean()
-{
-    static const bool clean = [] {
-        const char* env = getenv("PIRE_B200_LOOK_CLEAN");
-        return !(env && atoi(env) == 0);
-    }();
-    return clean;
-}
-
-// Two strings per lane (ScanUniformLook2Kernel) is the default shape of the look-ahead variant; PIRE_B200_LOOK_ILP=1
-// selects one string per lane (ScanUniformLookKernel).  PIRE_B200_LOOK_ILP_REGS=64|72|80 picks the register budget
-// and with it the CTA shape (two CTAs of 512 / 448 / 384 threads per SM).
-int LookIlp()
-{
-    static const int ilp = [] {
-        const char* env = getenv("PIRE_B200_LOOK_ILP");
-        return env && atoi(env) == 1 ? 1 : 2;
-    }();
-    return ilp;
-}
-int LookIlpRegs()
-{
-    static const int regs = [] {
-        const char* env = getenv("PIRE_B200_LOOK_ILP_REGS");
-        const int v = env ? atoi(env) : 72;
-        return v == 64 || v == 80 ? v : 72;
-    }();
-    return regs;
-}
-
-// The two-string look-ahead kernel is fed from the cp.async ring (ScanUniformLookRingKernel) unless PIRE_B200_LOOK_RING=0,
-// which selects the register-fed ScanUniformLook2Kernel; so does an explicit PIRE_B200_LOOK_ILP_REGS, which names one of its
-// register budgets.
-bool LookRing()
-{
-    static const bool ring = [] {
-        const char* env = getenv("PIRE_B200_LOOK_RING");
-        return !(env && atoi(env) == 0) && !getenv("PIRE_B200_LOOK_ILP_REGS");
-    }();
-    return ring;
-}
-
-// The one-string ring kernel keeps 8 slots per string in 16 warps; PIRE_B200_LOOK_RING1_SLOTS=6 selects 6 slots in 24
-// warps, the same 144 KB of ring per SM as the two-string kernel (experiments).
-// With per-string starts (pire_gpu_run_batch_from) every variant has one kernel, whatever the experiment switches above
-// say: the default shapes, 48 registers for the one-string look-ahead kernel and the ring for LOOK.  PRIV is run as PLAIN
-// by the caller.
-const void* StartsKernelFor(int variant, bool uniform)
-{
-    if (variant == kVariantLookRing1 && uniform)
-        return reinterpret_cast<const void*>(&ScanUniformLookRing1Kernel<kRing1Slots, true>);
-    if (variant == kVariantLook && uniform)
-        return reinterpret_cast<const void*>(&ScanUniformLookRingFromKernel);
-    if (variant == kVariantLook1 && uniform)
-        return reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 48, true, true>);
-    if (variant == kVariantLook64 && uniform)
-        return reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 48, false, true>);
-    if (uniform)
-        return variant == kVariantPred ? UniformKernelPtr<true, true>() : UniformKernelPtr<false, true>();
+    if (variant == kVariantPred)
+        return 1;
     if (variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1 || variant == kVariantLookRing1)
-        return GenericKernelPtr<2, true>();
-    return variant == kVariantPred ? GenericKernelPtr<1, true>() : GenericKernelPtr<0, true>();
+        return 2;
+    return 0;
 }
 
-const void* KernelFor(int variant, bool uniform, bool starts = false)
+// The kernel a batch of one variant runs and its launch shape.
+struct BatchKernel {
+    const void* fn;
+    int block;                  // threads per CTA
+    size_t ring_warp_bytes;     // each warp's input ring in shared memory, behind the tables
+    uint32_t units_per_step;    // units of 32 strings a warp takes at a time
+};
+
+template <typename K>
+const void* Fn(K* kernel) { return reinterpret_cast<const void*>(kernel); }
+
+// kStarts: the kernels that start every string from its own state (pire_gpu_run_batch_from).  PRIV has no such kernel:
+// with starts it is run as PLAIN.
+template <bool kStarts>
+BatchKernel BatchKernelOf(int variant, bool uniform)
 {
-    if (starts)
-        return StartsKernelFor(variant, uniform);
-    if (variant == kVariantPriv && uniform)
-        return reinterpret_cast<const void*>(&ScanUniformPrivKernel);
-    if (variant == kVariantLookRing1 && uniform)
-        return reinterpret_cast<const void*>(&ScanUniformLookRing1Kernel<kRing1Slots, false>);
-    if (variant == kVariantLook && uniform && LookIlp() == 2 && LookRing())
-        return reinterpret_cast<const void*>(&ScanUniformLookRingKernel);
-    if (variant == kVariantLook && uniform && LookIlp() == 2)
-        return LookIlpRegs() == 64   ? reinterpret_cast<const void*>(&ScanUniformLook2Kernel<64>)
-               : LookIlpRegs() == 80 ? reinterpret_cast<const void*>(&ScanUniformLook2Kernel<80>)
-                                     : reinterpret_cast<const void*>(&ScanUniformLook2Kernel<72>);
-    if ((variant == kVariantLook || variant == kVariantLook1) && uniform && LookClean())
-        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 48, true, false>)
-                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 40, true, false>);
-    if ((variant == kVariantLook || variant == kVariantLook1) && uniform)
-        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 48, false, false>)
-                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<false, 40, false, false>);
-    if (variant == kVariantLook64 && uniform)
-        return LookRegs() == 48 ? reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 48, false, false>)
-                                : reinterpret_cast<const void*>(&ScanUniformLookKernel<true, 40, false, false>);
-    if (uniform)
-        return variant == kVariantPred ? UniformKernelPtr<true>() : UniformKernelPtr<false>();
-    if (variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1 || variant == kVariantLookRing1)
-        return GenericKernelPtr<2>();         // CSR batches: one look-ahead kernel (32-slot filter)
-    return variant == kVariantPred ? GenericKernelPtr<1>() : GenericKernelPtr<0>();
+    const int mode = WalkMode(variant);
+    if (!uniform)
+        return {mode == 2 ? Fn(&ScanGenericKernel<2, kStarts>) : mode == 1 ? Fn(&ScanGenericKernel<1, kStarts>) : Fn(&ScanGenericKernel<0, kStarts>),
+                kBlock, 0, 1};
+    if (variant == kVariantPriv && !kStarts)
+        return {Fn(&ScanUniformPrivKernel), kPrivBlock, 0, 1};
+    if (variant == kVariantLook)
+        return {kStarts ? Fn(&ScanUniformLookRingFromKernel) : Fn(&ScanUniformLookRingKernel), kRingBlock, kRingWarpBytes, 2};
+    if (variant == kVariantLook1)
+        return {Fn(&ScanUniformLookKernel<false, 48, true, kStarts>), kLookBlock48, 0, 1};
+    if (variant == kVariantLook64)
+        return {Fn(&ScanUniformLookKernel<true, 48, false, kStarts>), kLookBlock48, 0, 1};
+    if (variant == kVariantLookRing1)
+        return {Fn(&ScanUniformLookRing1Kernel<kRing1Slots, kStarts>), kRing1Block, (size_t) kRing1Slots * kRing1SlotBytes, 1};
+    return {mode == 1 ? Fn(&ScanUniformKernel<true, kStarts>) : Fn(&ScanUniformKernel<false, kStarts>), kBlock, 0, 1};
+}
+
+BatchKernel BatchKernelFor(int variant, bool uniform, bool starts)
+{
+    return starts ? BatchKernelOf<true>(variant, uniform) : BatchKernelOf<false>(variant, uniform);
 }
 
 } // namespace
@@ -3636,13 +3472,13 @@ cudaError_t PrepareScanKernels(int device)
                         (int) kVariantLookRing1})
         for (bool uniform : {false, true})
             for (bool starts : {false, true}) {
-                err = cudaFuncSetAttribute(KernelFor(variant, uniform, starts), cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+                const void* fn = BatchKernelFor(variant, uniform, starts).fn;
+                err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
                 if (err != cudaSuccess)
                     return err;
                 // three CTAs of ~75 KB each per SM: ask for the largest shared-memory carve-out (kernels without a
                 // blocks-per-SM launch bound would otherwise get a smaller one and run two CTAs)
-                err = cudaFuncSetAttribute(KernelFor(variant, uniform, starts), cudaFuncAttributePreferredSharedMemoryCarveout,
-                                           cudaSharedmemCarveoutMaxShared);
+                err = cudaFuncSetAttribute(fn, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
                 if (err != cudaSuccess)
                     return err;
             }
@@ -3652,35 +3488,16 @@ cudaError_t PrepareScanKernels(int device)
 cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv_rows, int variant, bool uniform, LaunchPlan* plan,
                      bool starts)
 {
-    const bool priv = variant == kVariantPriv && uniform;
-    const bool look = variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1;
-    plan->block = priv ? kPrivBlock : (look && uniform) ? (LookRegs() == 48 ? kLookBlock48 : kLookBlock40) : kBlock;
-    if (look && uniform) {
-        static const int look_block = [] {
-            const char* env = getenv("PIRE_B200_LOOK_BLOCK");          // experiments: e.g. 640 = two CTAs of 20 warps at 48 registers
-            return env && atoi(env) >= 32 && atoi(env) <= 1024 && atoi(env) % 32 == 0 ? atoi(env) : 0;
-        }();
-        if (variant == kVariantLook && LookIlp() == 2)
-            plan->block = LookRing() ? kRingBlock : LookIlpRegs() == 64 ? 512 : LookIlpRegs() == 80 ? 384 : 448;
-        if (look_block)
-            plan->block = look_block;
-    }
-    if (variant == kVariantLookRing1 && uniform)
-        plan->block = kRing1Block;
-    // the kernels with per-string starts have the default shapes (StartsKernelFor)
-    const bool ring = variant == kVariantLook && uniform && (starts || (LookIlp() == 2 && LookRing()));
-    if (starts && look && uniform)
-        plan->block = ring ? kRingBlock : kLookBlock48;
+    const BatchKernel k = BatchKernelFor(variant, uniform, starts);
+    const bool priv = variant == kVariantPriv && uniform && !starts;
+    plan->block = k.block;
     plan->shared = priv ? ScanSharedBytes(hot_small, priv_rows) : uniform ? ScanSharedBytes(hot, 0) : GenericSharedBytes(hot);
-    if (ring)
-        plan->shared += (size_t) (plan->block / 32) * kRingWarpBytes;         // every warp's ring after the tables
-    if (variant == kVariantLookRing1 && uniform)
-        plan->shared += (size_t) (plan->block / 32) * kRing1Slots * kRing1SlotBytes;      // every warp's ring after the tables
+    plan->shared += (size_t) (plan->block / 32) * k.ring_warp_bytes;         // every warp's ring after the tables
     int sms = 0, per_sm = 0;
     cudaError_t err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
     if (err != cudaSuccess)
         return err;
-    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, KernelFor(variant, uniform, starts), plan->block, plan->shared);
+    err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, plan->block, plan->shared);
     if (err != cudaSuccess)
         return err;
     if (per_sm < 1)
@@ -3695,15 +3512,13 @@ cudaError_t LaunchScan(const ScanArgs& a, int variant, bool uniform, const Launc
 {
     if (a.n == 0)
         return cudaSuccess;
-    const bool starts = a.starts != nullptr;
-    uint64_t units = (a.n + 31) / 32;
-    if (variant == kVariantLook && uniform && (starts || LookIlp() == 2))
-        units = (units + 1) / 2;              // a warp of ScanUniformLook2Kernel / ScanUniformLookRing[From]Kernel takes two units at a time
+    const BatchKernel k = BatchKernelFor(variant, uniform, a.starts != nullptr);
+    const uint64_t units = ((a.n + 31) / 32 + k.units_per_step - 1) / k.units_per_step;
     const uint64_t warps_per_block = (uint64_t) plan.block / 32;
     uint64_t want = (units + warps_per_block - 1) / warps_per_block;
     int grid = (int) (want < (uint64_t) plan.grid ? want : (uint64_t) plan.grid);
     void* args[] = {const_cast<ScanArgs*>(&a)};
-    cudaError_t err = cudaLaunchKernel(KernelFor(variant, uniform, starts), dim3(grid), dim3(plan.block), args, plan.shared, stream);
+    cudaError_t err = cudaLaunchKernel(k.fn, dim3(grid), dim3(plan.block), args, plan.shared, stream);
     if (err == cudaSuccess)
         g_launches.fetch_add(1, std::memory_order_relaxed);
     return err;
@@ -3715,11 +3530,7 @@ cudaError_t LaunchSplit(const ScanArgs& a, int variant, int device, cudaStream_t
 {
     if (a.n == 0)
         return cudaSuccess;
-    static const uint32_t split_min = [] {
-        const char* env = getenv("PIRE_B200_SPLIT_MIN");          // experiments; a power of two keeps it a bucket boundary
-        return env && atoi(env) >= 64 ? (uint32_t) atoi(env) : kSplitMin;
-    }();
-    SplitCountKernel<<<1, 32, 0, stream>>>(a.offsets, a.order, a.n, split_min, const_cast<uint32_t*>(a.split_count), a.split_counter);
+    SplitCountKernel<<<1, 32, 0, stream>>>(a.offsets, a.order, a.n, kSplitMin, const_cast<uint32_t*>(a.split_count), a.split_counter);
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess)
         return err;
@@ -3759,10 +3570,6 @@ cudaError_t LaunchSplit(const ScanArgs& a, int variant, int device, cudaStream_t
 // down to 0, goes through the kernel.  a.string_ends / a.string_rounds are filled in here from per-call scratch.
 static cudaError_t LaunchStringGrid(const void* fn, const ScanArgs& a, size_t shared, int device, cudaStream_t stream)
 {
-    static const uint32_t min_blocks = [] {
-        const char* env = getenv("PIRE_B200_STRING_MIN_BLOCKS");  // experiments: 32-byte blocks per lane before CTAs are cut
-        return env && atoi(env) >= 1 ? (uint32_t) atoi(env) : kStringMinBlocks;
-    }();
     int optin = 0, sms = 0, per_sm = 0;
     cudaError_t err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
     if (err == cudaSuccess)
@@ -3776,7 +3583,7 @@ static cudaError_t LaunchStringGrid(const void* fn, const ScanArgs& a, size_t sh
     if (per_sm < 1)
         return cudaErrorLaunchOutOfResources;
     const uint64_t blocks = a.fixed_len / 32;
-    const uint64_t want = (blocks + (uint64_t) kBlock * min_blocks - 1) / ((uint64_t) kBlock * min_blocks);
+    const uint64_t want = (blocks + (uint64_t) kBlock * kStringMinBlocks - 1) / ((uint64_t) kBlock * kStringMinBlocks);
     const uint64_t full = (uint64_t) sms * (uint64_t) per_sm;
     const int grid = (int) (want < 1 ? 1 : want < full ? want : full);
     // rounds counters (3 words), then the warps' ends, double-buffered
@@ -3838,25 +3645,8 @@ cudaError_t LaunchPrefix(const ScanArgs& a, bool shortest, bool reverse, int dev
     if (err != cudaSuccess)
         return err;
     if (a.uniform && !reverse) {
-        // a.uniform: 1 = plain walk, 2 = exit filter
-        static const int block = [] {
-            const char* env = getenv("PIRE_B200_PREFIX_BLOCK");       // experiments; 640 = two CTAs of twenty warps at 48 registers
-            return env && atoi(env) >= 32 && atoi(env) <= 1024 && atoi(env) % 32 == 0 ? atoi(env) : 640;
-        }();
-        const bool pred = a.uniform == 2;
-        static const bool idp = [] {
-            const char* env = getenv("PIRE_B200_PREFIX_IDP");          // experiments: byte extraction on the FMA pipe
-            return env && atoi(env) != 0;
-        }();
-        if (pred)
-            fn = shortest ? reinterpret_cast<const void*>(&PrefixUniformKernel<true, true, false>)
-                          : reinterpret_cast<const void*>(&PrefixUniformKernel<false, true, false>);
-        else if (idp)
-            fn = shortest ? reinterpret_cast<const void*>(&PrefixUniformKernel<true, false, true>)
-                          : reinterpret_cast<const void*>(&PrefixUniformKernel<false, false, true>);
-        else
-            fn = shortest ? reinterpret_cast<const void*>(&PrefixUniformKernel<true, false, false>)
-                          : reinterpret_cast<const void*>(&PrefixUniformKernel<false, false, false>);
+        const int block = 640;                                         // two CTAs of twenty warps at 48 registers
+        fn = shortest ? reinterpret_cast<const void*>(&PrefixUniformKernel<true>) : reinterpret_cast<const void*>(&PrefixUniformKernel<false>);
         const size_t shared = ScanSharedBytes(a.hot, 0) + 272;
         int per_sm = 0;
         err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
@@ -3894,15 +3684,8 @@ cudaError_t LaunchLines(const ScanArgs& a, int variant, int device, cudaStream_t
 {
     if (a.n == 0)
         return cudaSuccess;
-    static const int forced = [] {
-        const char* env = getenv("PIRE_B200_LINES_KERNEL");        // experiments: 1 = pulling lanes, 2 = in stream
-        return env ? atoi(env) : 0;
-    }();
-    const bool in_stream = forced == 2 || (forced != 1 && a.start < a.hot);
-    if (in_stream && !(a.start < a.hot))
-        return cudaErrorInvalidValue;
-    const bool pred = variant == kVariantPred || variant == kVariantLook || variant == kVariantLook64 || variant == kVariantLook1
-                      || variant == kVariantLookRing1;
+    const bool in_stream = a.start < a.hot;
+    const bool pred = WalkMode(variant) != 0;
     const void* fn = in_stream ? (pred ? reinterpret_cast<const void*>(&ScanTextKernel<true>) : reinterpret_cast<const void*>(&ScanTextKernel<false>))
                                : (pred ? reinterpret_cast<const void*>(&ScanLinesKernel<true>) : reinterpret_cast<const void*>(&ScanLinesKernel<false>));
     const size_t shared = ScanSharedBytes(a.hot, 0) + (in_stream ? kTextFinBytes + kTextPackBytes : 0);
@@ -3920,22 +3703,14 @@ cudaError_t LaunchLines(const ScanArgs& a, int variant, int device, cudaStream_t
         return cudaErrorLaunchOutOfResources;
     ScanArgs tuned = a;
     int grid = sms * per_sm;
-    if (in_stream) {
-        tuned.text_segment = 0;                                        // chosen on the device from the text's size
-        if (const char* env = getenv("PIRE_B200_TEXT_SEGMENT"))       // experiments
-            tuned.text_segment = atoi(env) >= 32 && atoi(env) <= (1 << 20) ? (uint32_t) atoi(env) / 32u * 32u : tuned.text_segment;
-        // the persistent grid is launched whole: the number of units depends on the text's size, which only the device
-        // knows (offsets[n]); warps without a unit leave at once
-    } else {
+    // in stream, the persistent grid is launched whole: the number of units depends on the text's size, which only the
+    // device knows (offsets[n]); warps without a unit leave at once
+    if (!in_stream) {
         const uint64_t groups = (a.n + kLinesPerWarp - 1) / kLinesPerWarp;
         const uint64_t want = (groups + kWarpsPerBlock - 1) / kWarpsPerBlock;
         grid = (int) (want < (uint64_t) grid ? want : (uint64_t) grid);
         tuned.lines_turn = kPiecesPerTurn;
         tuned.lines_min_idle = kLinesMinIdle;
-        if (const char* env = getenv("PIRE_B200_LINES_TURN"))          // experiments
-            tuned.lines_turn = atoi(env) > 0 ? (uint32_t) atoi(env) : tuned.lines_turn;
-        if (const char* env = getenv("PIRE_B200_LINES_MIN_IDLE"))
-            tuned.lines_min_idle = atoi(env) > 0 ? (uint32_t) atoi(env) : tuned.lines_min_idle;
     }
     void* args[] = {&tuned};
     err = cudaLaunchKernel(fn, dim3(grid), dim3(kBlock), args, shared, stream);

@@ -64,7 +64,6 @@ struct ScanArgs {
     uint32_t* counts;            // n * regexps words, zeroed by the caller
     uint32_t lines_turn;         // lines kernel: chunks per lane between two hand-outs of lines
     uint32_t lines_min_idle;     // lines kernel: waiting lanes needed for a hand-out
-    uint32_t text_segment;       // in-stream lines kernel: bytes of text per lane and unit, a multiple of 32
     const uint64_t* weights;     // [states * count_words] packed per-state increments, or null
     uint32_t count_words;        // 0 = walk the accept lists, 1..2 = packed increments
     uint32_t count_always;       // final states are frequent: count every chunk, skip the look-ahead pass
@@ -102,8 +101,7 @@ constexpr int kVariantSlots = 8;      // size of per-variant arrays (variant ids
 
 size_t ScanSharedBytes(uint32_t hot, uint32_t priv_rows);
 cudaError_t PrepareScanKernels(int device);                       // raises the dynamic smem limit
-// starts: the plan of the kernel a launch with a.starts runs (the same as without, except for LOOK on uniform batches,
-// which then always runs the two-string ring kernel)
+// starts: the plan of the kernel a launch with a.starts runs (the same shape as without; PRIV has no such kernel)
 cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv_rows, int variant, bool uniform, LaunchPlan* plan,
                      bool starts = false);
 // a.starts selects the kernels that start every string from its own state

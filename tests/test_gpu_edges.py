@@ -1,18 +1,13 @@
 """The launch paths off the default shapes, against the in-repo oracle (oracle/pire_oracle.c, the plain byte-by-byte
 walk): start states outside the hot rows, hot sets of one to three rows, 32-bit transition tables, fixed-length
 batches that are not uniform (length not a multiple of 32, base not 32-byte aligned), writes past the last string,
-kernels that environment variables select, and strings past the 4 GiB mark.
+and strings past the 4 GiB mark.
 
 Every group first asserts the precondition that puts it on its path, so that a change to the hot order or to the
 dispatch cannot quietly move it off.  Every output buffer is larger than the batch and pre-filled with a sentinel:
-whatever lies past the last valid entry must still hold it afterwards.
-
-Run as a script (``python tests/test_gpu_edges.py env <setting>`` or ``lines-cold <json>``) the module is the child
-process of the tests whose kernels are chosen by environment variables, which the library reads once per process."""
+whatever lies past the last valid entry must still hold it afterwards."""
 import itertools
-import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -35,6 +30,16 @@ SENTINEL = 0x5A5A5A5A
 EXTRA = 64                       # entries past n in every output (and one more bitmap word)
 MARKS = ((True, True), (False, False), (True, False), (False, True))
 _SERIAL = itertools.count()
+
+
+def kernels_launched(fn):
+    """The names of the kernels that ``fn`` launches, space-separated, from torch.profiler."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        fn()
+        torch.cuda.synchronize()
+    return " ".join(e.name for e in prof.events())
 
 
 def is_uniform(corpus_ptr, offsets_ptr, fixed_len):
@@ -414,7 +419,7 @@ def test_cold_starts_and_tiny_hot_sets(name, cuda_device):
                     cold_seen["tuned" if tuned else "static"] += 1
                     lines_cases.append((max_hot, tuned, begin, end))
                     chk.sc.set_variant(4)
-                    if chk.sc.info().variant == 4:              # look-ahead set complete: ScanUniformLook2Kernel runs
+                    if chk.sc.info().variant == 4:              # look-ahead set complete: the LOOK ring kernel runs
                         cold_seen["look2"] += 1
                 label = "max_hot=%d %s%s" % (max_hot, "tuned" if tuned else "static", " cold" if cold else "")
                 for hb, what in zip(uniform, ("32B", "64B", "1KiB")):
@@ -432,46 +437,24 @@ def test_cold_starts_and_tiny_hot_sets(name, cuda_device):
     assert cold_seen["static"] >= 2 and cold_seen["tuned"] >= 1, cold_seen
     if name == "anchored":
         # tuned on text that dies at once, the hot id 0 is the dead state: the look-ahead set is complete with one hot
-        # row, and the two-strings-per-lane kernel starts its lanes cold
+        # row, and the LOOK ring kernel starts its lanes cold
         assert cold_seen["look2"] >= 1, cold_seen
-    # the lines runs of the cold configurations went through ScanLinesKernel: the in-stream kernel, forced, is refused
-    # for exactly those (LaunchLines), and accepted for a hot start
-    hot_case = (1, False, True, True)
-    out = run_child("lines-cold", {"PIRE_B200_LINES_KERNEL": "2"},
-                    json.dumps({"name": name, "cases": lines_cases + [hot_case], "seed": len(name)}))
-    refused = json.loads(out.split("REFUSED ", 1)[1].splitlines()[0])
-    assert refused == [True] * len(lines_cases) + [False], (lines_cases, refused)
-
-
-def _child_lines_cold(arg):
-    """Child of the cold-start test: for each (max_hot, tuned, begin, end), does pire_gpu_run_lines refuse the lines
-    batch?  PIRE_B200_LINES_KERNEL=2 forces the in-stream kernel, which needs a hot start."""
-    import pire_b200 as P
+    # the lines runs of the cold configurations went through ScanLinesKernel, and those of a hot start through the
+    # in-stream ScanTextKernel (LaunchLines)
     from pire_b200 import _native as N
-    cfg = json.loads(arg)
-    make_image, alphabet, literals = COLD_SCANNERS[cfg["name"]]
-    image = make_image()
-    rng = np.random.default_rng(cfg["seed"])
-    # the same draws as the parent, in the same order, up to the lines text and the tuning sample
-    for length in (32, 64, 1024):
-        random_rows(rng, 64 * 3 + 5, length, alphabet, literals)
-    random_strings(rng, alphabet, [0, 0, 1, 0] + list(rng.integers(0, 90, size=300)) + [0], literals)
-    random_strings(rng, alphabet, [8192, 8193, 9000, 12345, 20000] + list(rng.integers(0, 200, size=120)), literals)
-    lines = lines_batch(text_of_lines(rng, alphabet, literals, 1200, long_every=300))
-    tune_sample = random_strings(rng, alphabet, [64] * 64, literals)
-    refused = []
-    for max_hot, tuned, begin, end in cfg["cases"]:
+    hot_case = (1, False, True, True)
+    for case in lines_cases + [hot_case]:
+        max_hot, tuned, begin, end = case
         sc = P.Scanner(image, 0)
         sc.set_max_hot(max_hot)
         if tuned:
-            sc.Tune(P.Batch.from_strings(tune_sample), len(tune_sample), begin=not begin, end=not end)
-        n = lines.n
-        bits = _filled((n + 31) // 32 + 1)
-        rc = N.lib.pire_gpu_run_lines(sc._h, lines.corpus_ptr(), lines.offsets_ptr(), None, n,
-                                      (RUN_BEGIN if begin else 0) | (RUN_END if end else 0), bits.data_ptr(), None, None, _stream())
-        refused.append(rc != 0)
-    print("REFUSED " + json.dumps(refused))
-    return 0
+            sc.Tune(tune_batch, len(tune_sample), begin=not begin, end=not end)
+        bits = _filled((lines.n + 31) // 32 + 1)
+        flags = (RUN_BEGIN if begin else 0) | (RUN_END if end else 0)
+        launched = kernels_launched(lambda: N.check(N.lib.pire_gpu_run_lines(sc._h, lines.corpus_ptr(), lines.offsets_ptr(), None, lines.n, flags,
+                                                                             bits.data_ptr(), None, None, _stream()), "run_lines"))
+        want, other = ("ScanTextKernel", "ScanLinesKernel") if case == hot_case else ("ScanLinesKernel", "ScanTextKernel")
+        assert want in launched and other not in launched, (case, launched[:2000])
 
 
 # -------------------------------------------------------------------------------------------- (b) wide tables
@@ -588,72 +571,7 @@ def test_nothing_written_past_n(n, cuda_device):
         hf.count(csr_batch(random_strings(rng, b"abc de", list(rng.integers(0, 70, size=n)))), True, False, mode, "n=%d csr" % n)
 
 
-# -------------------------------------------------------------------------------- (e) environment-selected kernels
-
-ENV_SETTINGS = {
-    "look-clean-0": {"PIRE_B200_LOOK_CLEAN": "0"},
-    "look-regs-40": {"PIRE_B200_LOOK_REGS": "40"},
-    "look-ilp-1": {"PIRE_B200_LOOK_ILP": "1"},
-    "look-ilp-regs-64": {"PIRE_B200_LOOK_ILP_REGS": "64"},
-    "look-ilp-regs-80": {"PIRE_B200_LOOK_ILP_REGS": "80"},
-    "prefix-idp": {"PIRE_B200_PREFIX_IDP": "1"},
-    "prefix-pred": {"PIRE_B200_PREFIX_PRED": "1"},
-    "lines-kernel-0": {"PIRE_B200_LINES_KERNEL": "0"},
-    "lines-kernel-1": {"PIRE_B200_LINES_KERNEL": "1"},
-    "split-0": {"PIRE_B200_SPLIT": "0"},
-    "text-segment-32": {"PIRE_B200_TEXT_SEGMENT": "32"},
-    "text-segment-64": {"PIRE_B200_TEXT_SEGMENT": "64"},
-    "split-min-64": {"PIRE_B200_SPLIT_MIN": "64"},
-    "lines-turn-1": {"PIRE_B200_LINES_TURN": "1", "PIRE_B200_LINES_MIN_IDLE": "1"},
-}
-
-
-def run_child(kind, env_extra, arg, timeout=240):
-    env = dict(os.environ)
-    for k in [k for k in env if k.startswith("PIRE_B200_")]:
-        del env[k]
-    env.update(env_extra)
-    proc = subprocess.run([sys.executable, os.path.abspath(__file__), kind, arg], env=env, cwd=ROOT, capture_output=True,
-                          text=True, timeout=timeout)
-    assert proc.returncode == 0, "%s %s %s failed (%d):\n%s\n%s" % (kind, env_extra, arg, proc.returncode, proc.stdout[-3000:],
-                                                                    proc.stderr[-3000:])
-    return proc.stdout
-
-
-@pytest.mark.parametrize("setting", sorted(ENV_SETTINGS))
-def test_environment_selected_kernels(setting, cuda_device):
-    out = run_child("env", ENV_SETTINGS[setting], setting)
-    line = [l for l in out.splitlines() if l.startswith("EDGE-ENV ")]
-    assert line and line[-1] == "EDGE-ENV %s ok" % setting, out[-2000:]
-
-
-def _child_env(setting):
-    """One compact differential check of every entry point on glue10 and a small anchored pattern."""
-    rng = np.random.default_rng(7)
-    cases = [(glue10_image(), "glue10", GLUE10_ALPHABET, [b"GET ", b"error", b"timeout", b"(555) 123-4567"]),
-             (EDGE["anchored"]["image"], "anchored", ALPHABETS["anchored"], [b"abcde", b"cdabe"])]
-    for image, name, alphabet, literals in cases:
-        chk = Checker(image, name)
-        uniform = fixed_batch(random_rows(rng, 2000 + 7, 1024, alphabet, literals))
-        short = fixed_batch(random_rows(rng, 64 * 9 + 33, 64, alphabet, literals))
-        binned = csr_batch(random_strings(rng, alphabet, [8192, 9000, 20000, 70, 65, 64, 63] + list(rng.integers(0, 600, size=700)),
-                                          literals))
-        lines = lines_batch(text_of_lines(rng, alphabet, literals, 3000, long_every=700))
-        chk.all(uniform, setting + " uniform", marks=((True, True), (False, False)), suffix=False)
-        chk.all(short, setting + " uniform 64B", marks=((True, True),), prefix=False, suffix=False)
-        chk.all(binned, setting + " binned", marks=((True, True), (False, False)), variants=(1, 2, 4))
-        chk.all(lines, setting + " lines", marks=((True, True), (False, True)), variants=(1, 2), suffix=False)
-        for max_hot in (2, 1):
-            chk.sc.set_max_hot(max_hot)
-            chk.all(lines, "%s lines max_hot=%d" % (setting, max_hot), marks=((True, True), (False, False)), variants=(1, 2),
-                    prefix=False, suffix=False)
-            chk.all(binned, "%s binned max_hot=%d" % (setting, max_hot), marks=((False, True),), variants=(1, 2), prefix=False,
-                    suffix=False)
-    print("EDGE-ENV %s ok" % setting)
-    return 0
-
-
-# ----------------------------------------------------------------------------------------- (f) past 4 GiB
+# ----------------------------------------------------------------------------------------- (e) past 4 GiB
 
 def test_strings_past_4_gib(cuda_device):
     """A 4.3 GiB device buffer: a fixed-length batch (1000 bytes, not uniform), a CSR batch whose offsets pass 2^32
@@ -792,7 +710,3 @@ def test_strings_past_4_gib(cuda_device):
         torch.cuda.synchronize()
         torch.cuda.empty_cache()
 
-
-if __name__ == "__main__":
-    kind, arg = sys.argv[1], sys.argv[2]
-    sys.exit({"env": _child_env, "lines-cold": _child_lines_cold}[kind](arg))

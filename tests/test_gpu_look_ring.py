@@ -1,14 +1,8 @@
-"""The two-string look-ahead kernel fed from a cp.async ring (ScanUniformLookRingKernel) against the in-repo oracle and
-against the register-fed kernel it replaces (PIRE_B200_LOOK_RING=0 selects ScanUniformLook2Kernel).
+"""The two-string look-ahead kernel fed from a cp.async ring (ScanUniformLookRingKernel) against the in-repo oracle.
 
-Each kernel runs in a child process of its own, since the library reads the environment once per process: the child
-checks match bits, accept masks and StateIndex of every case against the oracle (with sentinels past n), saves the
-outputs, and the parent then asserts that both kernels wrote the same words.  Each child first profiles one launch and
-asserts that the kernel it means to test is the one that ran.
-
-Run as a script (``python tests/test_gpu_look_ring.py <out.npz>``) the module is that child."""
+Every case checks match bits, accept masks and StateIndex against the oracle, with sentinels past n.  One launch is
+profiled first, to assert that the ring kernel is the one that runs."""
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -22,8 +16,8 @@ for _p in (HERE, ROOT):
 
 from test_edge_images import ALPHABETS, EDGE, static_hot_order  # noqa: E402
 from test_gpu_edges import (EXTRA, GLUE10_ALPHABET, MARKS, RUN_BEGIN, RUN_END, BeginMark, Checker, HostBatch, _filled,  # noqa: E402
-                            _host, _stream, expect_equal, expect_untouched, fixed_batch, glue10_image, random_rows,
-                            random_strings, unpack_bits)
+                            _host, _stream, expect_equal, expect_untouched, fixed_batch, glue10_image, kernels_launched,
+                            random_rows, random_strings, unpack_bits)
 
 pytestmark = pytest.mark.gpu
 
@@ -31,9 +25,8 @@ RING_WARPS = 24                   # warps per CTA of ScanUniformLookRingKernel (
 HEADLINE_ALPHABET = b"abcdefghijklmnopqrstuvwxyz ABCDEFGHIJKLMNOPQRSTUVWXYZ0123456789.,:;-_/()[]{}@#"
 
 
-def run_look(chk, hb, begin, end, label, out):
-    """pire_gpu_run_batch with the look-ahead variant on a uniform batch; every output against the oracle, kept in
-    ``out`` under ``label`` for the comparison between the two kernels."""
+def run_look(chk, hb, begin, end, label):
+    """pire_gpu_run_batch with the look-ahead variant on a uniform batch; every output against the oracle."""
     from pire_b200 import _native as N
     assert hb.offsets is None and hb.fixed_len % 32 == 0 and hb.corpus_ptr() % 32 == 0, label      # a uniform batch
     chk.sc.set_variant(N.VARIANT_LOOK)
@@ -49,8 +42,6 @@ def run_look(chk, hb, begin, end, label, out):
     expect_equal(label, "StateIndex", hs[:n], s)
     expect_equal(label, "accept masks", hm[:n], m)
     expect_equal(label, "match bits", unpack_bits(label, hb_bits, n), f)
-    assert label not in out, label
-    out[label + " bits"], out[label + " masks"], out[label + " states"] = hb_bits, hm, hs
 
 
 def batch_at_allocation_end(rows):
@@ -67,15 +58,6 @@ def batch_at_allocation_end(rows):
     return hb
 
 
-def kernels_launched(fn):
-    import torch
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        fn()
-        torch.cuda.synchronize()
-    return " ".join(e.name for e in prof.events())
-
-
 def noexit_byte(host, begin):
     """A byte that sends the start state to a state no byte leaves (an anchored pattern that failed), and that state."""
     start = host.Next(host.Initialize(), BeginMark) if begin else host.Initialize()
@@ -86,21 +68,19 @@ def noexit_byte(host, begin):
     raise AssertionError("no byte reaches a NoExit state")
 
 
-def child(path):
+def test_ring_kernel_matches_oracle(cuda_device):
     import torch
     import pire_b200 as P
-    ring = os.environ.get("PIRE_B200_LOOK_RING") != "0"
     rng = np.random.default_rng(2024)
-    out = {}
-    # first of all, so that the caching allocator gives it a cudaMalloc of its own
+    # first of all, with the cache emptied, so that the caching allocator gives it a cudaMalloc of its own
+    torch.cuda.empty_cache()
     end_rows = random_rows(rng, 32 * 501 + 7, 1024, GLUE10_ALPHABET, [b"GET ", b"error", b"timeout"])
     at_end = batch_at_allocation_end(end_rows)
     at_end.device()
 
     glue = Checker(glue10_image(), "glue10")
-    launched = kernels_launched(lambda: run_look(glue, at_end, True, True, "probe", {}))
-    want_kernel = "ScanUniformLookRingKernel" if ring else "ScanUniformLook2Kernel"
-    assert want_kernel in launched and ("ScanUniformLookRingKernel" in launched) == ring, launched[:2000]
+    launched = kernels_launched(lambda: run_look(glue, at_end, True, True, "probe"))
+    assert "ScanUniformLookRingKernel" in launched, launched[:2000]
 
     from pire_b200 import workloads as W
     images = [("glue10", glue10_image(), GLUE10_ALPHABET, [b"GET ", b"error", b"timeout", b"(555) 123-4567"]),
@@ -121,12 +101,12 @@ def child(path):
                     assert chk.sc.info().tuned == 1
                 tag = "%s %s max_hot=%d" % (name, "tuned" if tuned else "static", max_hot)
                 for begin, end in MARKS:
-                    run_look(chk, own, begin, end, "%s own begin=%d end=%d" % (tag, begin, end), out)
+                    run_look(chk, own, begin, end, "%s own begin=%d end=%d" % (tag, begin, end))
                 if max_hot in (255, 2) and name == "glue10":
                     for length, n, hb in batches:
                         for begin, end in MARKS:
-                            run_look(chk, hb, begin, end, "%s len=%d n=%d begin=%d end=%d" % (tag, length, n, begin, end), out)
-                    run_look(chk, at_end, True, True, tag + " ends at the allocation's end", out)
+                            run_look(chk, hb, begin, end, "%s len=%d n=%d begin=%d end=%d" % (tag, length, n, begin, end))
+                    run_look(chk, at_end, True, True, tag + " ends at the allocation's end")
 
     # wide tables (32-bit cells): lanes leave the hot rows at once and are replayed block by block
     e = EDGE["wide"]
@@ -138,7 +118,7 @@ def child(path):
         chk.sc.set_max_hot(max_hot)
         assert chk.sc.info().table_bytes == chk.sc.info().states * chk.sc.info().letters * 4
         for begin, end in MARKS:
-            run_look(chk, wide, begin, end, "wide max_hot=%d begin=%d end=%d" % (max_hot, begin, end), out)
+            run_look(chk, wide, begin, end, "wide max_hot=%d begin=%d end=%d" % (max_hot, begin, end))
 
     # NoExit early exit, then a further pair of units on the same warp: the strings of every warp's first pair fall into
     # a state no byte leaves within their first block (the warp leaves after 64 of 128 bytes with two blocks still in
@@ -158,38 +138,6 @@ def child(path):
         rows[first:, :] = tokens[rng.integers(0, 2, size=(later, 64))].reshape(later, 128)
         rows[first::2, 127] = ord("e")
         chk = Checker(anchored, "anchored")
-        run_look(chk, fixed_batch(rows), begin, end, "NoExit exit, then another pair begin=%d end=%d" % (begin, end), out)
+        run_look(chk, fixed_batch(rows), begin, end, "NoExit exit, then another pair begin=%d end=%d" % (begin, end))
         _, _, states = chk.want(fixed_batch(rows[:64]), "run", begin, False)
         assert (states == dead).all()
-
-    np.savez_compressed(path, **out)
-    print("LOOK-RING %s ok %d" % ("ring" if ring else "look2", len(out)))
-    return 0
-
-
-def run_child(env_extra, path, timeout=900):
-    env = dict(os.environ)
-    for k in [k for k in env if k.startswith("PIRE_B200_")]:
-        del env[k]
-    env.update(env_extra)
-    proc = subprocess.run([sys.executable, os.path.abspath(__file__), path], env=env, cwd=ROOT, capture_output=True, text=True,
-                          timeout=timeout)
-    assert proc.returncode == 0, "%s failed (%d):\n%s\n%s" % (env_extra, proc.returncode, proc.stdout[-3000:], proc.stderr[-3000:])
-    return proc.stdout
-
-
-def test_ring_kernel_matches_oracle_and_register_kernel(cuda_device, tmp_path):
-    outs = {}
-    for key, env in (("ring", {}), ("look2", {"PIRE_B200_LOOK_RING": "0"})):
-        path = str(tmp_path / ("%s.npz" % key))
-        stdout = run_child(env, path)
-        assert "LOOK-RING %s ok" % key in stdout, stdout[-2000:]
-        outs[key] = np.load(path)
-    ring, look2 = outs["ring"], outs["look2"]
-    assert sorted(ring.files) == sorted(look2.files) and len(ring.files) > 300
-    for k in ring.files:
-        expect_equal(k, "output words", ring[k], look2[k])
-
-
-if __name__ == "__main__":
-    sys.exit(child(sys.argv[1]))

@@ -1019,10 +1019,10 @@ def test_host_entry_streams_chunks(cuda_device, ref, monkeypatch):
 
 
 @pytest.mark.parametrize("length", [32, 160, 1024])
-def test_uniform_bodies_of_prefix_and_count(length, cuda_device, ref, monkeypatch):
+def test_uniform_bodies_of_prefix_and_count(length, cuda_device, ref):
     """Fixed-length, 32-byte aligned batches take the register-streaming bodies of PrefixKernel / CountKernel (no
     staging ring).  Every mark combination, longest and shortest, a pattern with dead states, all counting modes:
-    equal to the reference and to the ring path on the same bytes."""
+    equal to the reference and to the ring path, which runs the same bytes as a CSR batch."""
     import torch
     import pire_b200 as P
     rng = np.random.default_rng(1000 + length)
@@ -1030,8 +1030,9 @@ def test_uniform_bodies_of_prefix_and_count(length, cuda_device, ref, monkeypatc
     host = rng.choice(np.frombuffer(b"abcx 01.", np.uint8), size=(n, length))
     host[::5, : min(length, 24)] = np.frombuffer((b"ab" * 12)[: min(length, 24)], np.uint8)
     host = np.ascontiguousarray(host).reshape(-1)
-    dev = torch.from_numpy(host).to("cuda:0")
+    dev = torch.from_numpy(np.concatenate([host, np.zeros(32, np.uint8)])).to("cuda:0")
     batch = P.Batch(dev, fixed_len=length, n=n)
+    csr = P.Batch(dev, offsets=torch.arange(0, (n + 1) * length, length, dtype=torch.int64, device="cuda:0"), n=n)
     for pat, opts in [(b"(ab)*c?", "n"), (b"a+b", ""), (rb"[0-9]+\.[0-9]+", ""), (b"[^x]*", "n")]:
         sc_ref = ref.compile(pat, opts)
         sc = P.Scanner(sc_ref.save(), cuda_device)
@@ -1040,12 +1041,9 @@ def test_uniform_bodies_of_prefix_and_count(length, cuda_device, ref, monkeypatc
                 for shortest in (False, True):
                     fn = P.ShortestPrefix if shortest else P.LongestPrefix
                     want = sc_ref.prefix(host, fixed_len=length, n=n, shortest=shortest, through_begin=tb, through_end=te, variant=2)
-                    monkeypatch.delenv("PIRE_B200_NO_UNIFORM_BODY", raising=False)
                     got = fn(sc, batch, throughBeginMark=tb, throughEndMark=te)
-                    monkeypatch.setenv("PIRE_B200_NO_UNIFORM_BODY", "1")
-                    ring = fn(sc, batch, throughBeginMark=tb, throughEndMark=te)
+                    ring = fn(sc, csr, throughBeginMark=tb, throughEndMark=te)
                     assert (got == want).all() and (ring == want).all(), (pat, tb, te, shortest)
-    monkeypatch.delenv("PIRE_B200_NO_UNIFORM_BODY", raising=False)
     for pat in (b"ab", b"[ab]+", b"a.*b|c"):
         hf = ref.compile_half_final(pat, "n", 0)
         sc = P.Scanner(hf.save(), cuda_device)
@@ -1054,5 +1052,6 @@ def test_uniform_bodies_of_prefix_and_count(length, cuda_device, ref, monkeypatc
                 want, wfin = hf.count(host, fixed_len=length, n=n, begin=begin, end=end)
                 for mode in (1, 2, 3):
                     sc.set_count_mode(mode)
-                    res = P.HalfFinalCount(sc, batch, begin=begin, end=end)
-                    assert (res.counts == want).all() and (res.final == wfin.astype(bool)).all(), (pat, begin, end, mode)
+                    for b in (batch, csr):
+                        res = P.HalfFinalCount(sc, b, begin=begin, end=end)
+                        assert (res.counts == want).all() and (res.final == wfin.astype(bool)).all(), (pat, begin, end, mode, b is csr)

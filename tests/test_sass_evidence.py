@@ -47,7 +47,7 @@ def test_only_hopper_code(kernels):
 
 
 def test_tables_are_staged_by_tma_and_walked_from_shared_memory(kernels):
-    for needle in ("ScanUniformKernel", "ScanUniformLook2Kernel", "ScanGenericKernel", "ScanSplitKernel", "ScanTextKernel",
+    for needle in ("ScanUniformKernel", "ScanGenericKernel", "ScanSplitKernel", "ScanTextKernel",
                    "PrefixKernel", "PrefixUniformKernel", "11CountKernel"):
         for text in pick(kernels, needle):
             assert count(text, r"\bUBLKCP") >= 1 and count(text, r"\bSYNCS") >= 1, needle       # cp.async.bulk + mbarrier
@@ -55,24 +55,10 @@ def test_tables_are_staged_by_tma_and_walked_from_shared_memory(kernels):
 
 
 def test_uniform_kernels_stream_with_128_bit_load_pairs_and_the_csr_kernels_with_ldgsts(kernels):
-    for needle in ("ScanUniformKernel", "ScanUniformLookKernel", "ScanUniformLook2Kernel", "PrefixUniformKernel", "ScanSplitKernel"):
+    for needle in ("ScanUniformKernel", "ScanUniformLookKernel", "PrefixUniformKernel", "ScanSplitKernel"):
         for text in pick(kernels, needle):
             assert count(text, r"\bLDG\.E\.[A-Z0-9.]*128") >= 4, needle                    # two per 32-byte sector
             assert count(text, r"\bLDGSTS") == 0, needle
     for text in pick(kernels, "ScanGenericKernel"):
         assert count(text, r"\bLDGSTS") >= 4
 
-
-def test_look_ahead_step_is_five_and_a_half_instructions(kernels):
-    """Per byte: IDP (byte + table base), SHF (probe), half an IMAD (clean bit of the even bytes), LOP3 -> predicate,
-    IMAD (row address), predicated LDS.U8: the walk's SHF count equals its predicated loads, half of them left shifts of
-    the bit-reversed filter, and there is about one LOP3 per step, not two."""
-    for text in pick(kernels, "ScanUniformLook2Kernel"):
-        steps = count(text, r"@!?P\d\s+LDS\.U8")
-        assert steps == 128                                              # 2 strings x 32 bytes x 2 ping-pong blocks
-        assert count(text, r"\bIDP\.4A") >= steps
-        assert steps // 2 <= count(text, r"\bSHF\.L\.W") <= steps // 2 + 8
-        assert steps // 2 <= count(text, r"\bSHF\.R\.W") <= steps // 2 + 16
-        assert count(text, r"\bLOP3") < steps + 40
-    for text in pick(kernels, "ScanUniformLookKernelILb0ELi48ELb0"):        # the six-instruction step kept for comparison
-        assert count(text, r"\bLOP3") > 2 * 64

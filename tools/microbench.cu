@@ -65,8 +65,8 @@ __device__ __forceinline__ void Ld32(const uint8_t* p, uint4& a, uint4& b)
 }
 __device__ __forceinline__ uint32_t Fold(uint4 v) { return v.x ^ v.y ^ v.z ^ v.w; }
 
-// The shipped load of ScanUniformLook2Kernel: two LDG.128 of one sector, both allocating in L1.  kL2 = 0, 64, 128 or
-// 256: the first load carries the L2 prefetch-size hint of that many bytes.
+// The load of the register-fed uniform kernels (ScanUniformKernel, ScanUniformLookKernel): two LDG.128 of one sector,
+// both allocating in L1.  kL2 = 0, 64, 128 or 256: the first load carries the L2 prefetch-size hint of that many bytes.
 template <int kL2>
 __device__ __forceinline__ void Ld32Pair(const uint8_t* p, uint4& a, uint4& b)
 {
@@ -89,7 +89,8 @@ __device__ __forceinline__ void Ld32Pair(const uint8_t* p, uint4& a, uint4& b)
 }
 
 // Two strings per lane (rows 64p + lane and 64p + 32 + lane), the next 32-byte block of both in flight while the
-// current one is folded: the input side of ScanUniformLook2Kernel without the walk.
+// current one is folded: the input side of the register-fed two-string look-ahead kernel (ScanUniformLook2Kernel, since
+// removed; the ring kernel replaced it) without the walk.
 template <int kL2>
 __global__ void __launch_bounds__(448) LoadPairKernel(const uint8_t* corpus, uint64_t n, uint32_t len, uint32_t* out)
 {
