@@ -275,7 +275,7 @@ class Checker:
                 lab = "%s [%s]" % (label, self.name)
                 if prefix:
                     self.prefix(hb, shortest, begin, end, lab)
-                if suffix and not hb.lines:
+                if suffix:
                     self.prefix(hb, shortest, begin, end, lab, suffix=True)
             for mode in count_modes:
                 self.count(hb, begin, end, mode, "%s [%s begin=%d end=%d]" % (label, self.name, begin, end))
@@ -433,7 +433,7 @@ def test_cold_starts_and_tiny_hot_sets(name, cuda_device):
                         chk.prefix(uniform[-1], shortest, begin, end, "%s uniform 1KiB [%s]" % (label, name))
                 chk.all(ragged, label + " csr", marks=((begin, end),))
                 chk.all(binned, label + " binned", marks=((begin, end),), variants=(1, 2, 4), prefix=False, suffix=False)
-                chk.all(lines, label + " lines", marks=((begin, end),), variants=(1, 2), suffix=False)
+                chk.all(lines, label + " lines", marks=((begin, end),), variants=(1, 2))
     assert cold_seen["static"] >= 2 and cold_seen["tuned"] >= 1, cold_seen
     if name == "anchored":
         # tuned on text that dies at once, the hot id 0 is the dead state: the look-ahead set is complete with one hot
@@ -481,7 +481,7 @@ def test_wide_tables(cuda_device):
         chk.all(uniform, label + " uniform", marks=((True, True), (False, False)))
         chk.all(ragged, label + " csr", marks=((True, True), (False, False)))
         chk.all(binned, label + " binned", marks=((True, True),), variants=(1, 2, 4), prefix=False, suffix=False)
-        chk.all(lines, label + " lines", marks=((True, True),), variants=(1, 2), suffix=False)
+        chk.all(lines, label + " lines", marks=((True, True),), variants=(1, 2))
         # the walks did leave the hot rows: most strings end in a state outside them (before the End mark)
         hot = static_hot(P.Scanner(e["image"], -1), max_hot)
         _, _, states = chk.want(uniform, "run", False, False)
@@ -563,7 +563,7 @@ def test_nothing_written_past_n(n, cuda_device):
     lines = lines_batch(text)
     assert lines.n == n
     for hb, what in ((uniform, "uniform"), (ragged, "csr"), (lines, "lines")):
-        chk.all(hb, "n=%d %s" % (n, what), marks=((True, True), (False, True)), suffix=not hb.lines)
+        chk.all(hb, "n=%d %s" % (n, what), marks=((True, True), (False, True)))
     hf = Checker(W.load_image("count_words5"), "count_words5")
     words = fixed_batch(random_rows(rng, n, 64, b"abc de"))
     for mode in (1, 2, 3):
