@@ -281,6 +281,42 @@ int pire_gpu_count_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uin
                           const uint32_t* d_start, uint64_t* d_counts,
                           uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
 
+/* HalfFinalScanner counts of many streams at once, each resumed from its own state ("how many times did each pattern
+ * occur in each of these connections / log tails / files read block by block").  Replaces, for every string i of a
+ * batch, the driver of tests/count_ut.cpp:54-63 with the state carried across calls the way a HalfFinalScanner::State is:
+ *     [sc.Initialize(st_i);]  [Pire::Step(sc, st_i, BeginMark);]  Pire::Run(sc, st_i, begin_i, end_i);  [Pire::Step(sc, st_i, EndMark);]
+ * One string per lane, on pire_gpu_count_batch's kernel.
+ *   Batch   CSR or fixed length, as in pire_gpu_run_batch.  n == 0 is a no-op that writes nothing.
+ *   flags   PIRE_GPU_RUN_BEGIN steps BeginMark from each string's own start and counts the state it reaches;
+ *           PIRE_GPU_RUN_END steps EndMark after the string's bytes and counts the state it reaches.  Anything else
+ *           (PIRE_GPU_RUN_LINES included) is PIRE_GPU_EINVAL.
+ *   Start   d_start == NULL: every string starts from Initialize(), whose TakeAction is counted (half_final.h:136-141), as
+ *           in pire_gpu_count_batch.  Otherwise d_start holds n StateIndex words in the reference's numbering; string i
+ *           resumes from d_start[i] and does NOT count it again (the call that reached it counted it).  A start >= Size()
+ *           reads no table and adds nothing; it yields match 0 and state 0xFFFFFFFF, and so stays in later rounds.  A
+ *           stream that joins in a later round takes pire_gpu_initial()'s StateIndex as its start word; its Initialize()
+ *           TakeAction is then not counted, which differs from a fresh start only when the initial state is final.
+ *   Counts  d_counts (required): n rows of max(1, RegexpsCount()) u64 counters, row i for string i, that the call ADDS
+ *           to -- like pire_gpu_count_string, unlike pire_gpu_count_batch, whose u32 rows are overwritten.  The caller
+ *           zeroes them before the first call.  Nothing past row n - 1 is written.
+ *   Chain   the d_state_idx of a call made without END is the d_start of the next call, and it may be the same buffer;
+ *           d_counts is the same buffer in every round.  Rounds update one state array and one counter array in place
+ *           with no synchronise in between, and the counts equal one call over each stream's concatenated pieces.  An
+ *           empty string passes its state through unchanged (and still takes the marks the flags ask for).
+ *   Output  each may be NULL: d_match_bits, Final() of each string's last state, packed (bits past n are 0);
+ *           d_state_idx, n words, its StateIndex (after End() with END).
+ * pire_gpu_scanner_set_count_mode is honoured; the results are identical in every mode.  With d_start == NULL and
+ * zeroed counters the counts are pire_gpu_count_batch's, widened to u64, and so are the match bits; match bits and
+ * states always equal pire_gpu_run_batch_from's on the same bytes and starts.  A NULL d_counts, a NULL corpus with
+ * non-empty strings and n > 2^40 are PIRE_GPU_EINVAL; a host-only handle gets PIRE_GPU_ENODEVICE.  Asynchronous on
+ * `stream`.  Not covered: ordered batches (d_order; the counting kernel has no length-binned launch) and line batches
+ * (no per-string starts, as in pire_gpu_run_batch_from). */
+int pire_gpu_count_batch_from(const pire_gpu_scanner* sc,
+                              const uint8_t* d_corpus, const uint64_t* d_offsets,
+                              uint64_t fixed_len, uint64_t n, uint32_t flags,
+                              const uint32_t* d_start, uint64_t* d_counts,
+                              uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
+
 /* The step before the path for line-oriented input (samples/pigrep/pigrep.cpp:38-45 calls
  * std::getline and then Runner(sc).Begin().Run(line).End() per line).
  * pire_gpu_split_lines finds the lines of a newline-delimited text resident in HBM:

@@ -337,6 +337,73 @@ private:
     bool Ran;
 };
 
+// StringCounter for n streams at once, one Pire::HalfFinalScanner::State each (pire_gpu_count_batch_from).  Every Run()
+// launches at once on a batch of n strings, string i the next piece of stream i; the states are carried in the
+// caller-owned device words d_state[0..n) and the counts ADDED to the caller-owned rows d_counts (n rows of
+// max(1, RegexpsCount()) u64, zeroed by the caller before the first call), so chained calls do not synchronise.  After
+// the stream is synchronised, d_counts[i * max(1, RegexpsCount()) + r] is stream i's State::Result(r), d_state[i] its
+// StateIndex and bit i % 32 of d_match_bits[i / 32] its Final().  End() is a launch of its own over n empty strings.
+//     BatchCounter c(gsc, n, d_counts, d_state);                                // Initialize(), counted
+//     BatchCounter c(gsc, BatchCounter::From(d_start), n, d_counts, d_state);   // resumed from d_start[i] (not counted again)
+//     c.Begin().Run(batch0).Run(batch1).End();
+class BatchCounter {
+public:
+    using StartWords = BatchRunner::StartWords;
+    static StartWords From(const uint32_t* d_start) { return StartWords(d_start); }
+
+    BatchCounter(const Scanner& sc, uint64_t n, uint64_t* d_counts, uint32_t* d_state, uint32_t* d_match_bits = nullptr,
+                 void* stream = nullptr)
+        : Sc(&sc), N(n), Start(nullptr), Counts(d_counts), State(d_state), Bits(d_match_bits), Stream(stream), Flags(0), Ran(false)
+    {
+        if (n != 0 && (!d_counts || !d_state))
+            throw Error(PIRE_GPU_EINVAL, "BatchCounter needs device words for its counters and its states");
+    }
+    // start.Words may be d_state: the states are then updated in place
+    BatchCounter(const Scanner& sc, StartWords start, uint64_t n, uint64_t* d_counts, uint32_t* d_state,
+                 uint32_t* d_match_bits = nullptr, void* stream = nullptr)
+        : BatchCounter(sc, n, d_counts, d_state, d_match_bits, stream)
+    {
+        if (n != 0 && !start.Words)
+            throw Error(PIRE_GPU_EINVAL, "BatchCounter::From needs device words");
+        Start = start.Words;
+    }
+
+    BatchCounter& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }
+    BatchCounter& Run(const Batch& b)
+    {
+        if (b.Count != N)
+            throw Error(PIRE_GPU_EINVAL, "BatchCounter::Run needs a batch of n strings");
+        Launch(b, 0);
+        return *this;
+    }
+    BatchCounter& End()
+    {
+        const Batch empty = {nullptr, nullptr, 0, N};
+        Launch(empty, PIRE_GPU_RUN_END);
+        return *this;
+    }
+
+private:
+    void Launch(const Batch& b, unsigned end)
+    {
+        Check(pire_gpu_count_batch_from(Sc->Raw(), b.Corpus, b.Offsets, b.FixedLen, b.Count, Flags | end, Ran ? State : Start,
+                                        Counts, Bits, State, Stream),
+              "pire_gpu_count_batch_from");
+        Flags = 0;
+        Ran = true;
+    }
+
+    const Scanner* Sc;
+    uint64_t N;
+    const uint32_t* Start;
+    uint64_t* Counts;
+    uint32_t* State;
+    uint32_t* Bits;
+    void* Stream;
+    unsigned Flags;
+    bool Ran;
+};
+
 // AcceptedRegexps for scanners with more than 32 regexps: rows of AcceptWords(sc) words, bit r of row i set iff
 // regexp r is accepted by the state string i stopped in (d_state_idx from BatchRunner::Launch).
 inline uint32_t AcceptWords(const Scanner& sc) { return pire_gpu_accept_words(sc.Raw()); }

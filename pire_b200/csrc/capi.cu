@@ -430,6 +430,24 @@ int pire_gpu_suffix_batch(const pire_gpu_scanner* sc, const uint8_t* d_corpus, c
     return PrefixOrSuffix(sc, d_corpus, d_offsets, fixed_len, n, flags, shortest, true, d_suffix_len, stream);
 }
 
+// The counting fields of every count entry point (HalfFinalScanner::TakeAction), count mode included.
+static void SetCounting(const pire_gpu_scanner* sc, ScanArgs* a, uint32_t flags)
+{
+    a->flags = sc->dev.flags;
+    a->end_class = sc->tab.end_class;
+    a->through_end = (flags & PIRE_GPU_RUN_END) ? 1 : 0;
+    a->acc_begin = sc->dev.acc_begin;
+    a->acc_ids = sc->dev.acc_ids;
+    a->first_final_hot = sc->tab.first_final_hot;
+    a->begin_class = sc->tab.begin_class;
+    a->initial = sc->tab.initial;
+    a->with_begin = (flags & PIRE_GPU_RUN_BEGIN) ? 1 : 0;
+    a->regexps = sc->dfa.regexps ? sc->dfa.regexps : 1;
+    a->weights = sc->dev.weights;
+    a->count_words = sc->count_mode == 1 ? 0 : sc->tab.count_words;
+    a->count_always = (sc->count_mode == 3 || (sc->count_mode == 0 && sc->final_share > 0.025)) ? 1 : 0;
+}
+
 int pire_gpu_count_batch(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,
                          uint64_t fixed_len, uint64_t n, uint32_t flags, uint32_t* d_counts, uint32_t* d_match_bits,
                          void* stream)
@@ -447,24 +465,43 @@ int pire_gpu_count_batch(const pire_gpu_scanner* sc, const uint8_t* d_corpus, co
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     ScanArgs a;
     FillArgs(sc, &a, d_corpus, d_offsets, fixed_len, n, flags);
-    a.flags = sc->dev.flags;
-    a.end_class = sc->tab.end_class;
-    a.through_end = (flags & PIRE_GPU_RUN_END) ? 1 : 0;
-    a.acc_begin = sc->dev.acc_begin;
-    a.acc_ids = sc->dev.acc_ids;
-    a.first_final_hot = sc->tab.first_final_hot;
-    a.begin_class = sc->tab.begin_class;
-    a.initial = sc->tab.initial;
-    a.with_begin = (flags & PIRE_GPU_RUN_BEGIN) ? 1 : 0;
-    a.regexps = sc->dfa.regexps ? sc->dfa.regexps : 1;
+    SetCounting(sc, &a, flags);
     a.counts = d_counts;
     a.match_bits = d_match_bits;
-    a.weights = sc->dev.weights;
-    a.count_words = sc->count_mode == 1 ? 0 : sc->tab.count_words;
-    a.count_always = (sc->count_mode == 3 || (sc->count_mode == 0 && sc->final_share > 0.025)) ? 1 : 0;
     a.uniform = IsUniform(d_corpus, d_offsets, fixed_len) ? 1 : 0;
     CUDA_TRY(cudaMemsetAsync(d_counts, 0, (size_t) n * a.regexps * 4, st));
     CUDA_TRY(LaunchCount(a, sc->device, st));
+    return PIRE_GPU_OK;
+}
+
+int pire_gpu_count_batch_from(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,
+                              uint64_t fixed_len, uint64_t n, uint32_t flags, const uint32_t* d_start, uint64_t* d_counts,
+                              uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream)
+{
+    int rc = CheckRunnable(sc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_count_batch_from takes PIRE_GPU_RUN_BEGIN and PIRE_GPU_RUN_END only");
+    if (n == 0)
+        return PIRE_GPU_OK;
+    if (!d_counts)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_count_batch_from needs n rows of max(1, regexps) u64 counters");
+    if (!d_corpus && (d_offsets || fixed_len != 0))
+        return Fail(PIRE_GPU_EINVAL, "null corpus with non-empty strings");
+    if (n > (1ull << 40))
+        return Fail(PIRE_GPU_EINVAL, "too many strings");
+    CUDA_TRY(cudaSetDevice(sc->device));
+    ScanArgs a;
+    FillArgs(sc, &a, d_corpus, d_offsets, fixed_len, n, flags);
+    SetCounting(sc, &a, flags);
+    if (d_start)
+        SetStarts(sc, &a, d_start, flags);
+    a.counts64 = reinterpret_cast<unsigned long long*>(d_counts);
+    a.match_bits = d_match_bits;
+    a.state_idx = d_state_idx;
+    a.uniform = IsUniform(d_corpus, d_offsets, fixed_len) ? 1 : 0;
+    CUDA_TRY(LaunchCount(a, sc->device, static_cast<cudaStream_t>(stream), true));
     return PIRE_GPU_OK;
 }
 
@@ -667,18 +704,7 @@ int pire_gpu_count_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uin
     a.begin_class = sc->tab.begin_class;
     a.match_bits = d_match_bits;
     a.state_idx = d_state_idx;
-    // the counting fields of pire_gpu_count_batch, count mode included
-    a.flags = sc->dev.flags;
-    a.end_class = sc->tab.end_class;
-    a.through_end = (flags & PIRE_GPU_RUN_END) ? 1 : 0;
-    a.acc_begin = sc->dev.acc_begin;
-    a.acc_ids = sc->dev.acc_ids;
-    a.first_final_hot = sc->tab.first_final_hot;
-    a.initial = sc->tab.initial;
-    a.regexps = sc->dfa.regexps ? sc->dfa.regexps : 1;
-    a.weights = sc->dev.weights;
-    a.count_words = sc->count_mode == 1 ? 0 : sc->tab.count_words;
-    a.count_always = (sc->count_mode == 3 || (sc->count_mode == 0 && sc->final_share > 0.025)) ? 1 : 0;
+    SetCounting(sc, &a, flags);
     a.counts64 = reinterpret_cast<unsigned long long*>(d_counts);
     a.count_rows = a.regexps <= kCountRowsMax ? 1 : 0;
     CUDA_TRY(LaunchCountString(a, sc->device, static_cast<cudaStream_t>(stream)));

@@ -77,7 +77,8 @@ struct ScanArgs {
     // mapped through new_of_old, BeginMark stepped when with_begin; one at or above `states` reports (0, 0, 0xFFFFFFFF).
     // starts may be state_idx: every kernel reads string i's start before it writes string i's state
     const uint32_t* starts;      // n words, or null: every string starts from `start`
-    // counting one string over the grid (pire_gpu_count_string): the counts are added to counts64 (max(1, regexps) words)
+    // counting one string over the grid (pire_gpu_count_string): the counts are added to counts64 (max(1, regexps) words);
+    // counting a batch from given states (pire_gpu_count_batch_from): n rows of max(1, regexps) words, row i string i's
     unsigned long long* counts64;
     uint32_t count_rows;         // 1: every warp sums into a row of u32 in shared memory first; 0: straight into counts64
 };
@@ -122,7 +123,10 @@ cudaError_t LaunchVisitCount(const ScanArgs& a, cudaStream_t stream);
 // prefix (left to right) or suffix (right to left) scan; a.with_begin/begin_class name the mark stepped first,
 // a.through_end/end_class the mark stepped last
 cudaError_t LaunchPrefix(const ScanArgs& a, bool shortest, bool reverse, int device, cudaStream_t stream);
-cudaError_t LaunchCount(const ScanArgs& a, int device, cudaStream_t stream);
+// HalfFinalScanner counts of a batch, one string per lane: into a.counts (n rows of u32, zeroed by the caller), or with
+// `from` (pire_gpu_count_batch_from) added to a.counts64 (n rows of u64), every string from a.starts[i] when a.starts is
+// given, its last state reported in a.match_bits / a.state_idx through a.fin
+cudaError_t LaunchCount(const ScanArgs& a, int device, cudaStream_t stream, bool from = false);
 // d_order <- string indices, longest half-octave length bucket first, corpus order inside a bucket (stable CUB radix sort).
 // stream-ordered scratch from the library's own per-device pool (see scan_kernels.cu)
 cudaError_t ScratchAlloc(void** out, size_t bytes, cudaStream_t stream);

@@ -503,6 +503,107 @@ class StringCounter:
         return bool(self._results()[1] & 1)
 
 
+class BatchCounter:
+    """``StringCounter`` for n streams at once (pire_gpu_count_batch_from): stream i's Pire::HalfFinalScanner state is
+    carried in a device tensor of n states and its counts added to row i of an (n, max(1, regexps)) device tensor of u64,
+    so a batch of streams arriving in pieces is counted round after round with no synchronise.  Every ``Run(batch)``
+    launches at once on the current stream; string i of the batch is the next piece of stream i.  ``states`` (an int32
+    CUDA tensor of n StateIndex values) resumes stream i from states[i] (not counted again: the run that reached it
+    counted it), None = Initialize() (counted).  ``Begin()`` is folded into the next launch, ``End()`` is a launch of its
+    own over n empty strings.  ``Counts()`` and ``StateTensor()`` do not synchronise; ``Result()``, ``AcceptedRegexps()``,
+    ``Final()``, ``Matches()`` and ``States()`` do."""
+
+    def __init__(self, sc, n, states=None):
+        torch = _torch()
+        self.Sc = sc
+        self.n = int(n)
+        dev = torch.device("cuda", sc.device)
+        if states is not None and (states.dtype != torch.int32 or not states.is_cuda or not states.is_contiguous()
+                                   or states.device != dev or states.numel() < self.n):
+            raise ValueError("states must be a contiguous int32 CUDA tensor of n states on the scanner's device")
+        self._start = states
+        self._states = torch.empty(self.n, dtype=torch.int32, device=dev)
+        self._bits = torch.empty((self.n + 31) // 32, dtype=torch.int32, device=dev)
+        self._counts = torch.zeros((self.n, max(1, sc.RegexpsCount())), dtype=torch.int64, device=dev)
+        self._begin = False
+        self._ran = False          # a launch has written the states
+
+    def Begin(self):
+        if self._ran:
+            raise ValueError("Begin() must precede Run()")
+        self._begin = True
+        return self
+
+    def Run(self, batch):
+        if batch.trim:
+            raise ValueError("line batches have no per-string starts")
+        if batch.order is not None:
+            raise ValueError("BatchCounter takes no length-ordered batch")
+        if batch.n != self.n:
+            raise ValueError("BatchCounter.Run needs a batch of n = %d strings, got %d" % (self.n, batch.n))
+        if batch.device != self._states.device:
+            raise ValueError("the batch must be on the scanner's device")
+        self._launch(batch.corpus.data_ptr(), None if batch.offsets is None else batch.offsets.data_ptr(), batch.fixed_len, 0)
+        return self
+
+    def End(self):
+        self._launch(None, None, 0, N.RUN_END)
+        return self
+
+    def _launch(self, corpus, offsets, fixed_len, flags):
+        if self._begin:
+            flags |= N.RUN_BEGIN
+            self._begin = False
+        torch = _torch()
+        if self._ran:
+            start = self._states.data_ptr()
+        else:
+            start = None if self._start is None else self._start.data_ptr()
+        stream = torch.cuda.current_stream(self._states.device).cuda_stream
+        N.check(N.lib.pire_gpu_count_batch_from(self.Sc._h, corpus, offsets, fixed_len, self.n, flags, start,
+                                                self._counts.data_ptr(), self._bits.data_ptr(), self._states.data_ptr(),
+                                                stream), "pire_gpu_count_batch_from")
+        self._ran = True
+
+    def _ensure(self):
+        if not self._ran:
+            self._launch(None, None, 0, 0)      # nothing run yet: the start states (after Begin() if it was asked for)
+
+    # without a synchronise ------------------------------------------------------------
+    def Counts(self):
+        """The device tensor (n, max(1, regexps)) of counters (int64 holding u64); row i is stream i's."""
+        self._ensure()
+        return self._counts
+
+    def StateTensor(self):
+        """The device tensor (int32, n) of the states reached, reference numbering: the ``states`` of a later
+        BatchCounter."""
+        self._ensure()
+        return self._states
+
+    # synchronising --------------------------------------------------------------------
+    def Result(self, i, regexp_id):
+        """State::Result(regexp_id) of stream i (half_final.h:88-90)."""
+        return int(self.Counts()[i, regexp_id].item())
+
+    def AcceptedRegexps(self, i):
+        """HalfFinalScanner::AcceptedRegexps (half_final.h:130-133) of stream i: regexps with a non-zero counter."""
+        return [int(r) for r in np.nonzero(self.Counts()[i].cpu().numpy())[0]]
+
+    def Matches(self):
+        """numpy bool[n]: Final() of each stream's state."""
+        self._ensure()
+        words = self._bits.cpu().numpy().view(np.uint32)
+        return np.unpackbits(words.view(np.uint8), bitorder="little")[: self.n].astype(bool)
+
+    def Final(self, i):
+        return bool(self.Matches()[i])
+
+    def States(self):
+        """StateIndex() of each stream's state (reference numbering); 0xFFFFFFFF for a start outside the scanner."""
+        return self.StateTensor().cpu().numpy().view(np.uint32)
+
+
 def Runner(sc, states=None):
     """Pire::Runner(sc) (run.h:388-389); with ``states`` Pire::Runner(sc, st) (run.h:391-392) for every string."""
     return RunHelper(sc, states)

@@ -228,5 +228,27 @@ sc.run_batch(bb, N.RUN_BEGIN | N.RUN_END, None, None, st, start_idx=st)
 want = [run_from(orc, np.frombuffer(s, np.uint8), int(x), True, True)[2] for s, x in zip(strings, starts)]
 assert (st.cpu().numpy().view(np.uint32) == np.array(want, np.uint32)).all()
 print("ok run_batch_from", flush=True)
+# HalfFinalScanner counts of many streams (pire_gpu_count_batch_from): a ragged CSR batch cut into two rounds, chained in
+# place through one state array and one counts array (some starts outside the scanner), in every count mode, against
+# one count over the whole strings
+from count_oracle import count_from
+img = W.load_image("hf_glue10")
+orc = Oracle(img)
+sc = P.Scanner(img, 0)
+strings = [bytes(rng.choice(np.frombuffer(b"GET error timeout https:// ab", np.uint8), size=int(k))) for k in rng.integers(0, 400, size=70)]
+cuts = [int(rng.integers(0, len(s) + 1)) for s in strings]
+starts = rng.integers(0, sc.Size(), size=len(strings))
+starts[5] = sc.Size()
+for mode in (1, 2, 3):
+    sc.set_count_mode(mode)
+    st = torch.from_numpy(starts.astype(np.int32)).to(dev)
+    c = P.BatchCounter(sc, len(strings), st).Begin()
+    for k in (0, 1):
+        c.Run(P.Batch.from_strings([s[:x] if k == 0 else s[x:] for s, x in zip(strings, cuts)]))
+    c.End()
+    got = c.Counts().cpu().numpy()
+    for i, s in enumerate(strings):
+        assert got[i].tolist() == count_from(orc, np.frombuffer(s, np.uint8), int(starts[i]))[0], (mode, i)
+print("ok count_batch_from", flush=True)
 torch.cuda.synchronize()
 print("sanitize_run done, launches:", N.lib.pire_gpu_launch_count())
