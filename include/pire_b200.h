@@ -281,6 +281,36 @@ int pire_gpu_count_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uin
                           const uint32_t* d_start, uint64_t* d_counts,
                           uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
 
+/* Where the HalfFinalScanner matches end in one long string, with the whole GPU ("regexp 3 occurs 41 times in this log:
+ * where?").  pire_gpu_count_string's run, listing every count it would add instead of adding it: each TakeAction
+ * (half_final.h:154-163) yields one entry (end, id) for each id in the accept list of the state entered, in list order
+ * (a state that lists an id twice yields two entries, as it adds two to the count).
+ *   Input, flags, start and chain   exactly as in pire_gpu_count_string: BEGIN and/or END (anything else, LINES
+ *           included, is PIRE_GPU_EINVAL); d_start == NULL is Initialize(), whose TakeAction is reported; a resumed
+ *           start is not reported again; a start >= Size() reports nothing and yields match 0 and state 0xFFFFFFFF;
+ *           d_state_idx may be d_start.
+ *   end     base + the number of text bytes consumed when the state was entered: Initialize() and BeginMark are at
+ *           base + 0, byte k of the text at base + k + 1, EndMark at base + n_bytes.
+ *   Order   walk order: ascending end, and within one end in step order, then accept-list order.  The order is fully
+ *           determined, so two calls on the same input write identical arrays.
+ *   Output  *d_found (required) is one device u64 that the call reads and ADDS its number of entries to.  The call's
+ *           k-th entry goes to index *d_found + k of d_ends (end) and d_ids (regexp id) if that index is < capacity;
+ *           nothing at or past capacity and nothing below the incoming *d_found is written.  d_ends and d_ids may each
+ *           be NULL (nothing goes to a NULL array).  With too small a buffer the written entries are exactly the first
+ *           `capacity` entries of the full answer, and *d_found is still the full total, so the caller can tell and call
+ *           again with a larger buffer.  d_match_bits[0] / d_state_idx[0] as in pire_gpu_count_string.
+ *   Chain   zero *d_found once and pass the running byte offset as `base`: chained calls append, with no synchronise
+ *           in between, and write what one call over the concatenated text writes.
+ * The entries with id == r number exactly pire_gpu_count_string's Result(r) on the same bytes, flags and start; match
+ * and state equal pire_gpu_run_string's.  pire_gpu_scanner_set_count_mode does not apply.  A NULL d_found and a NULL
+ * d_text with n_bytes > 0 are PIRE_GPU_EINVAL; a host-only handle gets PIRE_GPU_ENODEVICE.  Asynchronous on `stream`;
+ * re-entrant across streams on one handle (per-call scratch).  It costs about pire_gpu_count_string plus one more walk
+ * of the bytes and the writes of the entries (DESIGN.md 4). */
+int pire_gpu_match_ends_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uint64_t n_bytes, uint32_t flags,
+                               const uint32_t* d_start, uint64_t base,
+                               uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity, uint64_t* d_found,
+                               uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
+
 /* HalfFinalScanner counts of many streams at once, each resumed from its own state ("how many times did each pattern
  * occur in each of these connections / log tails / files read block by block").  Replaces, for every string i of a
  * batch, the driver of tests/count_ut.cpp:54-63 with the state carried across calls the way a HalfFinalScanner::State is:

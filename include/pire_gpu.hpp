@@ -337,6 +337,69 @@ private:
     bool Ran;
 };
 
+// Where the matches StringCounter counts end (pire_gpu_match_ends_string): StringCounter's shape, with the entries
+// (end, regexp id) appended in walk order to the caller-owned device arrays d_ends / d_ids (either may be null) of
+// `capacity` entries, and their number ADDED to the caller-owned device word *d_found (zeroed by the caller before the
+// first call).  Run() may be called many times: the pieces are one string, the state carried in d_state and the running
+// byte offset kept here, so an end is the number of bytes of all pieces consumed when the state was entered, and chained
+// calls do not synchronise.  End() is a launch of its own, at the total length.  After the stream is synchronised,
+// *d_found is the number of entries (all of them, even past capacity) and the first min(*d_found, capacity) entries of
+// d_ends / d_ids are the answer's first ones.
+//     StringMatchEnds m(gsc, d_ends, d_ids, capacity, d_found, d_state);                                  // Initialize()
+//     StringMatchEnds m(gsc, StringMatchEnds::From(d_start), d_ends, d_ids, capacity, d_found, d_state);  // resumed
+//     m.Begin().Run(d_a, n_a).Run(d_b, n_b).End();
+class StringMatchEnds {
+public:
+    using StartWord = StringRunner::StartWord;
+    static StartWord From(const uint32_t* d_start) { return StartWord(d_start); }
+
+    StringMatchEnds(const Scanner& sc, uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity, uint64_t* d_found, uint32_t* d_state,
+                    uint32_t* d_match_bits = nullptr, void* stream = nullptr)
+        : Sc(&sc), Start(nullptr), Ends(d_ends), Ids(d_ids), Capacity(capacity), Found(d_found), State(d_state), Bits(d_match_bits),
+          Stream(stream), Base(0), Flags(0), Ran(false)
+    {
+        if (!d_found || !d_state)
+            throw Error(PIRE_GPU_EINVAL, "StringMatchEnds needs device words for the number of entries and the state");
+    }
+    // start.Word may be d_state: the state is then updated in place
+    StringMatchEnds(const Scanner& sc, StartWord start, uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity, uint64_t* d_found,
+                    uint32_t* d_state, uint32_t* d_match_bits = nullptr, void* stream = nullptr)
+        : StringMatchEnds(sc, d_ends, d_ids, capacity, d_found, d_state, d_match_bits, stream)
+    {
+        if (!start.Word)
+            throw Error(PIRE_GPU_EINVAL, "StringMatchEnds::From needs a device word");
+        Start = start.Word;
+    }
+
+    StringMatchEnds& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }
+    StringMatchEnds& Run(const uint8_t* d_text, uint64_t n) { Launch(d_text, n, 0); return *this; }
+    StringMatchEnds& End() { Launch(nullptr, 0, PIRE_GPU_RUN_END); return *this; }
+
+private:
+    void Launch(const uint8_t* d_text, uint64_t n, unsigned end)
+    {
+        Check(pire_gpu_match_ends_string(Sc->Raw(), d_text, n, Flags | end, Ran ? State : Start, Base, Ends, Ids, Capacity, Found,
+                                         Bits, State, Stream),
+              "pire_gpu_match_ends_string");
+        Base += n;
+        Flags = 0;
+        Ran = true;
+    }
+
+    const Scanner* Sc;
+    const uint32_t* Start;
+    uint64_t* Ends;
+    uint32_t* Ids;
+    uint64_t Capacity;
+    uint64_t* Found;
+    uint32_t* State;
+    uint32_t* Bits;
+    void* Stream;
+    uint64_t Base;
+    unsigned Flags;
+    bool Ran;
+};
+
 // StringCounter for n streams at once, one Pire::HalfFinalScanner::State each (pire_gpu_count_batch_from).  Every Run()
 // launches at once on a batch of n strings, string i the next piece of stream i; the states are carried in the
 // caller-owned device words d_state[0..n) and the counts ADDED to the caller-owned rows d_counts (n rows of

@@ -711,6 +711,37 @@ int pire_gpu_count_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uin
     return PIRE_GPU_OK;
 }
 
+int pire_gpu_match_ends_string(const pire_gpu_scanner* sc, const uint8_t* d_text, uint64_t n_bytes, uint32_t flags,
+                               const uint32_t* d_start, uint64_t base, uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity,
+                               uint64_t* d_found, uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream)
+{
+    int rc = CheckRunnable(sc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_match_ends_string takes PIRE_GPU_RUN_BEGIN and PIRE_GPU_RUN_END only");
+    if (!d_found)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_match_ends_string needs a device word for the number of entries");
+    if (!d_text && n_bytes)
+        return Fail(PIRE_GPU_EINVAL, "null text with n_bytes > 0");
+    CUDA_TRY(cudaSetDevice(sc->device));
+    ScanArgs a;
+    FillArgs(sc, &a, d_text, nullptr, n_bytes, 1, flags);
+    a.start_idx = d_start;
+    a.new_of_old = sc->dev.new_of_old;
+    a.states = sc->tab.states;
+    a.match_bits = d_match_bits;
+    a.state_idx = d_state_idx;
+    SetCounting(sc, &a, flags);
+    a.ends = d_ends;
+    a.ids = d_ids;
+    a.ends_capacity = capacity;
+    a.found = reinterpret_cast<unsigned long long*>(d_found);
+    a.ends_base = base;
+    CUDA_TRY(LaunchMatchEndsString(a, sc->device, static_cast<cudaStream_t>(stream)));
+    return PIRE_GPU_OK;
+}
+
 int pire_gpu_scanner_tune(pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,
                           uint64_t fixed_len, uint64_t n_sample, uint32_t flags, void* stream)
 {

@@ -3362,6 +3362,324 @@ __global__ void __launch_bounds__(kBlock, kStringBlocksPerSM) CountStringKernel(
     }
 }
 
+// ---------------------------------------------------------------- where the matches end in one string over the whole grid
+//
+// pire_gpu_match_ends_string: every TakeAction of HalfFinalScanner (half_final.h:154-163) on one string as entries
+// (position, regexp id), in walk order.  One cooperative launch of CountStringKernel's grid and pieces, in four phases:
+//   1. Locate: CountStringKernel's phase 1 unchanged.  After its last grid.sync() every lane knows the true state at the
+//      start of its piece.
+//   2. Count: every lane walks its piece from there and counts its entries (EndsLane<false>).  A 16-step running maximum
+//      of hot ids skips every chunk that enters no final state (CountChunk16's test); a chunk that does is walked again
+//      through the hot rows, adding the list lengths staged in shared memory, or through the complete table when it
+//      leaves the hot rows.  The grid's first lane adds Initialize(), BeginMark and the head, its last lane the tail and
+//      EndMark, and the last lane reports the match and the state.
+//   3. Scan: an exclusive prefix sum of the lane totals in lane order, which is the order of the text, over the grid: a
+//      block scan, every CTA's total published to scratch, grid.sync(), every CTA adds up the totals of the CTAs before it.
+//   4. Emit: every lane whose slice begins below the capacity walks its piece once more (EndsLane<true>) and writes its
+//      entries into its slice, up to its last entry or the capacity, whichever comes first.
+// The scan places the entries, where atomics appending them would not: the arrays are the same on every run, and a
+// buffer too small for the answer holds its first `capacity` entries.
+
+// The entries of the states a walk enters: counted (kWrite false: n is the count), or written from index n on, up to
+// index `stop` (kWrite: the end of the lane's slice or the capacity).
+template <bool kWrite>
+struct EndsSink {
+    uint64_t n;
+    uint64_t stop;
+
+    __device__ __forceinline__ bool Full() const { return kWrite && n >= stop; }
+    // s a full state, entered when `pos` bytes of the call's text had been consumed
+    __device__ __forceinline__ void Take(const ScanArgs& a, const Tables& t, uint32_t s, uint64_t pos)
+    {
+        const bool final = s < t.H ? s >= a.first_final_hot : (__ldg(a.flags + s) & 1u) != 0;
+        if (!final)
+            return;
+        uint32_t k = __ldg(a.acc_begin + s);
+        const uint32_t e = __ldg(a.acc_begin + s + 1);
+        if (!kWrite) {
+            n += e - k;
+            return;
+        }
+        for (; k < e && n < stop; ++k, ++n) {
+            if (a.ends)
+                a.ends[n] = a.ends_base + pos;
+            if (a.ids)
+                a.ids[n] = __ldg(a.acc_ids + k);
+        }
+    }
+};
+
+// 16 bytes at position `at` of the text.  Counting adds the hot list lengths of a chunk that stays in the hot rows
+// without a table read per step; writing needs each final state's list, so it takes every chunk with a final state
+// through the complete table (whose hot rows are the shared ones, SlowStep).
+template <bool kWrite>
+__device__ __forceinline__ void EndsChunk16(const ScanArgs& a, const Tables& t, const uint32_t* hot_len, LaneState& s, uint4 v,
+                                            uint64_t at, EndsSink<kWrite>& o)
+{
+    const uint32_t before = s.g;
+    uint32_t g = before, top = 0;
+#pragma unroll
+    for (int w = 0; w < 4; ++w) {
+        const uint32_t word = w == 0 ? v.x : w == 1 ? v.y : w == 2 ? v.z : v.w;
+        FastStep<false>(t, g, word, 0x5540);
+        top = max(top, g);
+        FastStep<false>(t, g, word, 0x5541);
+        top = max(top, g);
+        FastStep<false>(t, g, word, 0x5542);
+        top = max(top, g);
+        FastStep<false>(t, g, word, 0x5543);
+        top = max(top, g);
+    }
+    if (top < a.first_final_hot) {           // sixteen steps through non-final hot states: no entry
+        s.g = g;
+        return;
+    }
+    if (!kWrite && top < t.H) {
+        // every step in the hot rows (the sink is the highest id), some in final ones: their list lengths
+        uint32_t add = 0;
+        g = before;
+#pragma unroll
+        for (int w = 0; w < 4; ++w) {
+            const uint32_t word = w == 0 ? v.x : w == 1 ? v.y : w == 2 ? v.z : v.w;
+#pragma unroll
+            for (int b = 0; b < 4; ++b) {
+                FastStep<false>(t, g, word, 0x5540 + b);
+                add += hot_len[g];
+            }
+        }
+        o.n += add;
+        s.g = g;
+        return;
+    }
+    uint32_t full = before == t.H ? s.cold : before;
+    EdgeBytes eb(v, 0);
+    for (int k = 0; k < 16; ++k) {
+        full = SlowStep(t, full, eb.Next());
+        o.Take(a, t, full, at + k + 1);
+    }
+    SetFull(t, s, full);
+}
+
+// One lane's share of the string, walked by phase 2 (kWrite false) and again by phase 4 (kWrite): Initialize(),
+// BeginMark and the head (the grid's first lane), the piece from its true start `start_full`, the tail and EndMark (the
+// last lane).  Returns the state after the lane's bytes (before EndMark).  A writing walk stops when its sink is full.
+template <bool kWrite>
+__device__ __forceinline__ uint32_t EndsLane(const ScanArgs& a, const Tables& t, const uint32_t* hot_len, uint32_t start,
+                                             uint32_t start_full, bool first, bool last, const uint8_t* body,
+                                             const uint8_t* piece, uint32_t my_blocks, EndsSink<kWrite>& o)
+{
+    const uint8_t* const end = a.corpus + a.fixed_len;
+    if (first) {
+        // Initialize() ends in TakeAction (half_final.h:136-141); a resumed run reported its start in the previous call.
+        // `start` is the state after BeginMark when it was asked for.
+        if (!a.start_idx)
+            o.Take(a, t, a.initial, 0);
+        if (a.with_begin)
+            o.Take(a, t, start, 0);
+        uint32_t full = start;
+        for (const uint8_t* p = a.corpus; p < body; ++p) {
+            full = SlowStep(t, full, *p);
+            o.Take(a, t, full, (uint64_t) (p - a.corpus) + 1);
+        }
+    }
+    LaneState s;
+    SetFull(t, s, start_full);
+    if (my_blocks != 0 && !o.Full()) {
+        // CountStringKernel's loop: 32-byte loads one block ahead in registers
+        const uint32_t len = 32u * my_blocks;
+        const uint64_t at = (uint64_t) (piece - a.corpus);
+        uint4 a0, a1, b0, b1;
+        LoadStream32(piece, a0, a1);
+        for (uint32_t off = 0;;) {
+            off += 32;
+            const bool more_b = off < len;
+            if (more_b)
+                LoadStream32(piece + off, b0, b1);
+            EndsChunk16<kWrite>(a, t, hot_len, s, a0, at + off - 32, o);
+            EndsChunk16<kWrite>(a, t, hot_len, s, a1, at + off - 16, o);
+            if (!more_b || o.Full())
+                break;
+            off += 32;
+            const bool more_a = off < len;
+            if (more_a)
+                LoadStream32(piece + off, a0, a1);
+            EndsChunk16<kWrite>(a, t, hot_len, s, b0, at + off - 32, o);
+            EndsChunk16<kWrite>(a, t, hot_len, s, b1, at + off - 16, o);
+            if (!more_a || o.Full())
+                break;
+        }
+    }
+    uint32_t full = FullState(t, s);
+    if (last && !o.Full()) {
+        for (const uint8_t* p = piece + 32 * (size_t) my_blocks; p < end; ++p) {      // the last piece ends the body
+            full = SlowStep(t, full, *p);
+            o.Take(a, t, full, (uint64_t) (p - a.corpus) + 1);
+        }
+        if (a.through_end)
+            o.Take(a, t, FullNext(t, full, a.end_class), a.fixed_len);      // Step(EndMark)
+    }
+    return full;
+}
+
+__global__ void __launch_bounds__(kBlock, kStringBlocksPerSM) MatchEndsStringKernel(const __grid_constant__ ScanArgs a)
+{
+    namespace cg = cooperative_groups;
+    cg::grid_group grid = cg::this_grid();
+    uint8_t* const smem = pire_b200_smem;
+    SharedView sv = CarveShared(smem, a.hot);
+    StageTables(a, sv, a.hot8, a.hot);
+    // behind the marks: the scan's words (every warp's entries, the CTA's first entry, *a.found as the call found it),
+    // then the accept-list length of every hot state (0 for the non-final ones)
+    unsigned long long* const sums = reinterpret_cast<unsigned long long*>(sv.stage + kSplitMarkBytes);
+    uint32_t* const hot_len = reinterpret_cast<uint32_t*>(sums + kWarpsPerBlock + 2);
+    for (uint32_t i = threadIdx.x; i < a.hot; i += blockDim.x)
+        hot_len[i] = i >= a.first_final_hot ? __ldg(a.acc_begin + i + 1) - __ldg(a.acc_begin + i) : 0u;
+    if (threadIdx.x == 0)
+        sums[kWarpsPerBlock + 1] = *a.found;       // read before the first grid.sync(), written after the last
+    __syncthreads();
+
+    Tables t;
+    t.hot = sv.hot;
+    t.base = SmemAddr(sv.hot);
+    t.cls = sv.cls;
+    t.full = a.full;
+    t.H = a.hot;
+    t.letters = a.letters;
+    t.wide = a.wide;
+    t.m0 = a.exit_bitmap0;
+
+    // the true start, as in ScanStringKernel (*a.start_idx may be the output word: written only after a grid.sync())
+    uint32_t start = a.start;
+    bool valid = true;
+    if (a.start_idx)
+        StartFrom(a, t, *a.start_idx, start, valid);
+    const bool skip = !valid || (start < t.H && sv.noexit[start] != 0);       // multi.h:955-958: no byte leaves it
+
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t warp = blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
+    const uint32_t warps = gridDim.x * kWarpsPerBlock;
+    uint8_t* const marks = sv.stage + (threadIdx.x >> 5) * (32 * kSplitMarks) + lane;
+    const uintptr_t buf_lo = reinterpret_cast<uintptr_t>(a.corpus);
+    const uintptr_t buf_hi = buf_lo + a.fixed_len;
+    const uint8_t* const end = a.corpus + a.fixed_len;
+
+    // phase 1, locate: CountStringKernel's
+    LaneState s;
+    SetFull(t, s, start);
+    if (warp == 0 && !skip) {
+        const uint8_t* p = a.corpus;
+        const uint32_t mis = (uint32_t) (buf_lo & 15);
+        if (p < end && mis != 0) {
+            const uint64_t room = (uint64_t) (end - p);
+            const uint32_t nhead = room < 16 - mis ? (uint32_t) room : 16 - mis;
+            EdgeFast<false>(t, s, EdgeBytes(LoadChunk16(p - mis, buf_lo, buf_hi), mis).Words(), nhead);
+            p += nhead;
+        }
+        if ((reinterpret_cast<uintptr_t>(p) & 16) && end - p >= 16)
+            Chunk16<false>(t, s, LoadEdge16(p));
+    }
+    const uint8_t* const body = StringBody(a.corpus, end);
+    const uint32_t blocks_total = (reinterpret_cast<uintptr_t>(body) & 31) ? 0u : (uint32_t) ((end - body) >> 5);
+    const uint32_t lanes = gridDim.x * kBlock;
+    const uint32_t me = blockIdx.x * kBlock + threadIdx.x;
+    const uint32_t base = blocks_total / lanes, rem = blocks_total % lanes;
+    const uint32_t my_blocks = base + (me < rem ? 1u : 0u);
+    const uint64_t my_first = (uint64_t) me * base + (me < rem ? me : rem);
+    const uint32_t trips = base + (rem ? 1u : 0u);
+    const uint32_t per_mark = (trips + kSplitMarks - 1) / kSplitMarks;
+    const uint8_t* const piece = body + 32 * my_first;
+    const uint32_t first_start = __shfl_sync(0xffffffffu, FullState(t, s), 0);
+
+    uint32_t start_full = me == 0 ? first_start : 0u;
+    uint32_t end_full = start_full;
+    if (!skip) {
+        SetFull(t, s, start_full);
+        WalkPiece<false>(t, s, piece, my_blocks, trips, per_mark, marks, 0);
+        end_full = FullState(t, s);
+
+        uint4 head0 = make_uint4(0, 0, 0, 0), head1 = head0;
+        bool head_fresh = my_blocks != 0;
+        if (head_fresh)
+            LoadStream32P(piece, head0, head1);
+        PIRE_B200_STITCH_GRID(false);
+    } else {
+        grid.sync();
+    }
+    if (!valid) {
+        // a start outside the scanner reads no table and reports nothing: match 0, state 0xFFFFFFFF, *a.found unchanged
+        if (me == lanes - 1) {
+            if (a.match_bits)
+                a.match_bits[0] = 0;
+            if (a.state_idx)
+                a.state_idx[0] = 0xFFFFFFFFu;
+        }
+        return;
+    }
+    if (skip)
+        start_full = start;  // a NoExit start: every piece starts (and stays) there, and each of its steps is reported
+
+    // phase 2, count
+    const bool first = me == 0, last = me == lanes - 1;
+    EndsSink<false> count{0, 0};
+    const uint32_t fin = EndsLane<false>(a, t, hot_len, start, start_full, first, last, body, piece, my_blocks, count);
+    if (last) {
+        const DeviceFin f = a.fin[fin];
+        if (a.match_bits)
+            a.match_bits[0] = f.result >> 31;
+        if (a.state_idx)
+            a.state_idx[0] = f.result & 0x7fffffffu;
+    }
+
+    // phase 3, scan: inclusive in the warp, the warps' totals in the CTA, the CTAs' totals over the grid
+    uint64_t x = count.n;
+#pragma unroll
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+        const uint64_t y = __shfl_up_sync(0xffffffffu, x, d);
+        if (lane >= d)
+            x += y;
+    }
+    if (lane == 31)
+        sums[threadIdx.x >> 5] = x;
+    __syncthreads();
+    if (threadIdx.x < 32) {
+        const uint64_t own = lane < kWarpsPerBlock ? sums[lane] : 0;
+        uint64_t w = own;
+#pragma unroll
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+            const uint64_t y = __shfl_up_sync(0xffffffffu, w, d);
+            if (lane >= d)
+                w += y;
+        }
+        if (lane < kWarpsPerBlock)
+            sums[lane] = w - own;                   // the warp's first entry in the CTA
+        if (lane == 31)
+            __stcg(a.string_sums + blockIdx.x, (unsigned long long) w);
+    }
+    grid.sync();
+    if (threadIdx.x < 32) {
+        uint64_t before = 0;
+        for (uint32_t c = lane; c < blockIdx.x; c += 32)
+            before += __ldcg(a.string_sums + c);
+#pragma unroll
+        for (uint32_t d = 16; d >= 1; d >>= 1)
+            before += __shfl_xor_sync(0xffffffffu, before, d);
+        if (lane == 0) {
+            const uint64_t found = sums[kWarpsPerBlock + 1];
+            sums[kWarpsPerBlock] = found + before;  // the CTA's first entry
+            if (blockIdx.x == gridDim.x - 1)
+                *a.found = found + before + __ldcg(a.string_sums + blockIdx.x);
+        }
+    }
+    __syncthreads();
+
+    // phase 4, emit: the lane's slice is [first entry, first entry + count.n)
+    const uint64_t from = sums[kWarpsPerBlock] + sums[threadIdx.x >> 5] + (x - count.n);
+    if (count.n == 0 || from >= a.ends_capacity)
+        return;
+    EndsSink<true> out{from, from + count.n < a.ends_capacity ? from + count.n : a.ends_capacity};
+    EndsLane<true>(a, t, hot_len, start, start_full, first, last, body, piece, my_blocks, out);
+}
+
 // Visit counter for pire_gpu_scanner_tune: how many input bytes are consumed in
 // each state (new numbering).  Run-length compressed so that a lane resting in
 // one state issues one atomic per stay, not one per byte.
@@ -3617,8 +3935,10 @@ cudaError_t LaunchSplit(const ScanArgs& a, int variant, int device, cudaStream_t
 
 // One string (a.corpus, a.fixed_len bytes) over the persistent grid (ScanStringKernel, CountStringKernel).  The grid is the occupancy
 // query's, cut to one CTA per kBlock * kStringMinBlocks blocks of body so that pieces do not get short; every length,
-// down to 0, goes through the kernel.  a.string_ends / a.string_rounds are filled in here from per-call scratch.
-static cudaError_t LaunchStringGrid(const void* fn, const ScanArgs& a, size_t shared, int device, cudaStream_t stream)
+// down to 0, goes through the kernel.  a.string_ends / a.string_rounds (and with `sums`, a.string_sums) are filled in
+// here from per-call scratch.
+static cudaError_t LaunchStringGrid(const void* fn, const ScanArgs& a, size_t shared, int device, cudaStream_t stream,
+                                    bool sums = false)
 {
     int optin = 0, sms = 0, per_sm = 0;
     cudaError_t err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
@@ -3636,9 +3956,9 @@ static cudaError_t LaunchStringGrid(const void* fn, const ScanArgs& a, size_t sh
     const uint64_t want = (blocks + (uint64_t) kBlock * kStringMinBlocks - 1) / ((uint64_t) kBlock * kStringMinBlocks);
     const uint64_t full = (uint64_t) sms * (uint64_t) per_sm;
     const int grid = (int) (want < 1 ? 1 : want < full ? want : full);
-    // rounds counters (3 words), then the warps' ends, double-buffered
+    // rounds counters (3 words), then the warps' ends, double-buffered, then (sums) one u64 per CTA
     uint32_t* scratch = nullptr;
-    const size_t words = 4 + 2 * (size_t) grid * kWarpsPerBlock;
+    const size_t words = 4 + 2 * (size_t) grid * kWarpsPerBlock + (sums ? 2 * (size_t) grid : 0);
     err = ScratchAlloc(reinterpret_cast<void**>(&scratch), words * 4, stream);
     if (err != cudaSuccess)
         return err;
@@ -3646,6 +3966,8 @@ static cudaError_t LaunchStringGrid(const void* fn, const ScanArgs& a, size_t sh
     ScanArgs with_scratch = a;
     with_scratch.string_rounds = scratch;
     with_scratch.string_ends = scratch + 4;
+    if (sums)
+        with_scratch.string_sums = reinterpret_cast<unsigned long long*>(scratch + 4 + 2 * (size_t) grid * kWarpsPerBlock);
     void* args[] = {&with_scratch};
     if (err == cudaSuccess)
         err = cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(kBlock), args, shared, stream);
@@ -3676,6 +3998,13 @@ cudaError_t LaunchCountString(const ScanArgs& a, int device, cudaStream_t stream
     const size_t shared = ScanSharedBytes(a.hot, 0) + kSplitMarkBytes + (size_t) (a.hot + 1) * a.count_words * 8
                           + (a.count_rows ? (size_t) kWarpsPerBlock * a.regexps * 4 : 0);
     return LaunchStringGrid(fn, a, shared, device, stream);
+}
+
+// Behind the tables and the marks: the scan's words (kWarpsPerBlock + 2 u64), then the hot states' list lengths.
+cudaError_t LaunchMatchEndsString(const ScanArgs& a, int device, cudaStream_t stream)
+{
+    const size_t shared = ScanSharedBytes(a.hot, 0) + kSplitMarkBytes + (kWarpsPerBlock + 2) * 8 + (size_t) a.hot * 4;
+    return LaunchStringGrid(reinterpret_cast<const void*>(&MatchEndsStringKernel), a, shared, device, stream, true);
 }
 
 cudaError_t LaunchPrefix(const ScanArgs& a, bool shortest, bool reverse, int device, cudaStream_t stream)

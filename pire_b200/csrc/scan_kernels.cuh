@@ -81,6 +81,14 @@ struct ScanArgs {
     // counting a batch from given states (pire_gpu_count_batch_from): n rows of max(1, regexps) words, row i string i's
     unsigned long long* counts64;
     uint32_t count_rows;         // 1: every warp sums into a row of u32 in shared memory first; 0: straight into counts64
+    // where the matches end in one string over the grid (pire_gpu_match_ends_string): the call's entry k goes to index
+    // *found + k of ends / ids when that is below ends_capacity; *found is read once and advanced by the call's total
+    uint64_t* ends;              // ends_base + bytes consumed when a final state was entered, or null
+    uint32_t* ids;               // the regexp id of each entry, or null
+    uint64_t ends_capacity;      // entries of ends / ids
+    unsigned long long* found;   // one word, read and added to
+    uint64_t ends_base;          // position of the text's first byte in the caller's numbering
+    unsigned long long* string_sums; // scratch: each CTA's number of entries
 };
 
 struct LaunchPlan {
@@ -119,6 +127,9 @@ cudaError_t LaunchString(const ScanArgs& a, int variant, int device, cudaStream_
 cudaError_t LaunchCountString(const ScanArgs& a, int device, cudaStream_t stream);
 // the largest max(1, regexps) for which LaunchCountString keeps a row of counters per warp in shared memory
 constexpr uint32_t kCountRowsMax = 256;
+// Every TakeAction of HalfFinalScanner on one string over the whole grid (MatchEndsStringKernel): LaunchString's grid and
+// pieces, SetCounting's accept lists, the entries in walk order from index *a.found on, *a.found advanced by their number
+cudaError_t LaunchMatchEndsString(const ScanArgs& a, int device, cudaStream_t stream);
 cudaError_t LaunchVisitCount(const ScanArgs& a, cudaStream_t stream);
 // prefix (left to right) or suffix (right to left) scan; a.with_begin/begin_class name the mark stepped first,
 // a.through_end/end_class the mark stepped last

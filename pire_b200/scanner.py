@@ -503,6 +503,113 @@ class StringCounter:
         return bool(self._results()[1] & 1)
 
 
+class StringMatchEnds:
+    """Where the matches ``StringCounter`` counts end (pire_gpu_match_ends_string): one entry (end, regexp id) for every
+    count, in walk order, where end is the number of bytes consumed (over all ``Run()`` calls) when the final state was
+    entered.  The entries go to device tensors of ``capacity`` entries; ``FoundTensor()`` counts all of them, even past
+    the capacity, whose entries are dropped (the written ones are then the answer's first ``capacity``).  ``Run(text)``
+    may be called many times with no synchronise: the state is carried in a device word and the running byte offset on
+    the host.  ``state`` = a StateIndex to resume from (not reported again), None = Initialize() (reported).
+    ``Begin()`` is folded into the first launch, ``End()`` is a launch of its own.  ``EndsTensor()``, ``IdsTensor()`` and
+    ``FoundTensor()`` do not synchronise; ``Found()``, ``Ends()``, ``Ids()``, ``Final()`` and ``State()`` do."""
+
+    def __init__(self, sc, capacity, state=None):
+        self.Sc = sc
+        self.capacity = int(capacity)
+        self._start = None if state is None else int(state)
+        self._words = None         # device: [StateIndex, match word]
+        self._ends = self._ids = self._found = None
+        self._base = 0             # bytes run so far
+        self._begin = False
+        self._ran = False
+
+    def Begin(self):
+        if self._ran:
+            raise ValueError("Begin() must precede Run()")
+        self._begin = True
+        return self
+
+    def Run(self, text):
+        torch = _torch()
+        if text.dtype != torch.uint8 or not text.is_cuda or not text.is_contiguous() or text.device.index != self.Sc.device:
+            raise ValueError("text must be a contiguous uint8 CUDA tensor on the scanner's device")
+        self._launch(text, 0)
+        return self
+
+    def End(self):
+        self._launch(None, N.RUN_END)
+        return self
+
+    def _launch(self, text, flags):
+        if self._begin:
+            flags |= N.RUN_BEGIN
+            self._begin = False
+        start = stream = words = ends = ids = found = None
+        if self.Sc.device >= 0:
+            torch = _torch()
+            dev = torch.device("cuda", self.Sc.device)
+            if self._words is None:
+                self._words = torch.empty(2, dtype=torch.int32, device=dev)
+                self._ends = torch.empty(self.capacity, dtype=torch.int64, device=dev)
+                self._ids = torch.empty(self.capacity, dtype=torch.int32, device=dev)
+                self._found = torch.zeros(1, dtype=torch.int64, device=dev)
+                if self._start is not None:
+                    word = self._start & 0xFFFFFFFF
+                    self._words[0] = word - (1 << 32) if word >= (1 << 31) else word
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            if self._ran or self._start is not None:
+                start = self._words.data_ptr()
+            words, ends, ids, found = self._words.data_ptr(), self._ends.data_ptr(), self._ids.data_ptr(), self._found.data_ptr()
+        n = 0 if text is None else text.numel()
+        N.check(N.lib.pire_gpu_match_ends_string(self.Sc._h, None if text is None else text.data_ptr(), n, flags, start, self._base,
+                                                 ends, ids, self.capacity, found, None if words is None else words + 4, words,
+                                                 stream), "pire_gpu_match_ends_string")
+        self._base += n
+        self._ran = True
+
+    def _ready(self):
+        if not self._ran:
+            self._launch(None, 0)          # nothing run yet: the start state itself (after Begin() if it was asked for)
+
+    def EndsTensor(self):
+        """The device tensor of ends (int64 holding u64), ``capacity`` long; does not synchronise."""
+        self._ready()
+        return self._ends
+
+    def IdsTensor(self):
+        """The device tensor of regexp ids (int32 holding u32), ``capacity`` long; does not synchronise."""
+        self._ready()
+        return self._ids
+
+    def FoundTensor(self):
+        """The device word (int64 holding u64) counting every entry, also those past the capacity; does not synchronise."""
+        self._ready()
+        return self._found
+
+    def Found(self):
+        """The number of entries, also those past the capacity."""
+        return int(self.FoundTensor().item())
+
+    def Ends(self):
+        """The first min(Found(), capacity) ends, as numpy u64."""
+        k = min(self.Found(), self.capacity)
+        return self._ends[:k].cpu().numpy().view(np.uint64)
+
+    def Ids(self):
+        """The first min(Found(), capacity) regexp ids, as numpy u32."""
+        k = min(self.Found(), self.capacity)
+        return self._ids[:k].cpu().numpy().view(np.uint32)
+
+    def State(self):
+        """StateIndex() of the state reached (reference numbering); 0xFFFFFFFF for a start outside the scanner."""
+        self._ready()
+        return int(self._words.cpu().numpy().view(np.uint32)[0])
+
+    def Final(self):
+        self._ready()
+        return bool(self._words.cpu().numpy().view(np.uint32)[1] & 1)
+
+
 class BatchCounter:
     """``StringCounter`` for n streams at once (pire_gpu_count_batch_from): stream i's Pire::HalfFinalScanner state is
     carried in a device tensor of n states and its counts added to row i of an (n, max(1, regexps)) device tensor of u64,

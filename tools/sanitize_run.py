@@ -250,5 +250,17 @@ for mode in (1, 2, 3):
     for i, s in enumerate(strings):
         assert got[i].tolist() == count_from(orc, np.frombuffer(s, np.uint8), int(starts[i]))[0], (mode, i)
 print("ok count_batch_from", flush=True)
+# where the matches end in one string (pire_gpu_match_ends_string): three chained pieces, one cut inside a 32-byte block,
+# into a buffer too small for the answer, against count_string on the same bytes and a call with room for all of it
+sc.set_count_mode(0)
+text = torch.from_numpy(rng.choice(np.frombuffer(b"GET error timeout https:// ab", np.uint8), size=300_007)).to(dev)
+cnt = P.StringCounter(sc).Begin().Run(text).End()
+total = sum(cnt.Result(r) for r in range(max(1, sc.RegexpsCount())))
+full = P.StringMatchEnds(sc, total).Begin().Run(text).End()
+part = P.StringMatchEnds(sc, total // 2).Begin().Run(text[:5]).Run(text[5:100_003]).Run(text[100_003:]).End()
+assert full.Found() == part.Found() == total
+assert (part.Ends() == full.Ends()[: total // 2]).all() and (part.Ids() == full.Ids()[: total // 2]).all()
+assert np.bincount(full.Ids(), minlength=max(1, sc.RegexpsCount())).tolist() == [cnt.Result(r) for r in range(max(1, sc.RegexpsCount()))]
+print("ok match_ends_string", flush=True)
 torch.cuda.synchronize()
 print("sanitize_run done, launches:", N.lib.pire_gpu_launch_count())
