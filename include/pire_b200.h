@@ -347,6 +347,42 @@ int pire_gpu_count_batch_from(const pire_gpu_scanner* sc,
                               const uint32_t* d_start, uint64_t* d_counts,
                               uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
 
+/* Where the HalfFinalScanner matches end in many streams at once, each resumed from its own state ("regexp 3 occurred 41
+ * times in stream 17: where?").  pire_gpu_count_batch_from's run, listing every count it would add instead of adding it:
+ * each TakeAction of string i yields one entry (i, end, id) for each id in the accept list of the state entered, in list
+ * order.  One string per lane, on pire_gpu_count_batch_from's kernel, in two walks around a scan of the strings' totals.
+ *   Batch, flags, start and chain   exactly as in pire_gpu_count_batch_from: CSR or fixed length; BEGIN and/or END
+ *           (anything else, LINES included, is PIRE_GPU_EINVAL); d_start == NULL is Initialize(), whose TakeAction is
+ *           reported; a resumed start is not reported again; a start >= Size() reports nothing and yields match 0 and
+ *           state 0xFFFFFFFF; d_state_idx may be d_start.
+ *   Positions d_pos (n u64 words, or NULL: every base 0 and nothing written): d_pos[i] is the number of bytes stream i
+ *           consumed before this call, the `base` of pire_gpu_match_ends_string.  Initialize() and BeginMark are at
+ *           d_pos[i] + 0, byte k of string i at d_pos[i] + k + 1, EndMark at d_pos[i] + len_i.  The call adds len_i to
+ *           d_pos[i] (also for an unknown start), so rounds chain with no host work.
+ *   Order   by string index, then walk order within a string: ascending end, then step order, then accept-list order.
+ *   Output  *d_found (required) is one device u64 that the call reads and ADDS its number of entries to.  The call's
+ *           k-th entry goes to index *d_found + k of d_strings (string index), d_ends (end) and d_ids (regexp id) if that
+ *           index is < capacity; nothing at or past capacity and nothing below the incoming *d_found is written.  Each of
+ *           the three arrays may be NULL.  With too small a buffer the written entries are exactly the first `capacity`
+ *           entries of the full answer, and *d_found is still the full total.  The placement comes from a scan, not from
+ *           atomics: two calls on the same input write identical bytes.  d_match_bits / d_state_idx (each may be NULL)
+ *           as in pire_gpu_count_batch_from.
+ *   Chain   zero *d_found and d_pos once; the d_state_idx of a call made without END is the d_start of the next, and
+ *           may be the same buffer.  Rounds append with no synchronise in between, and write what one call over each
+ *           stream's concatenated pieces writes.
+ * The entries of string i are what pire_gpu_match_ends_string writes for string i alone, with start d_start[i] (or
+ * NULL) and base d_pos[i]; their per-id histogram is row i of pire_gpu_count_batch_from; match bits and states equal
+ * pire_gpu_run_batch_from's.  pire_gpu_scanner_set_count_mode does not apply.  n == 0 is a no-op that writes nothing.  A
+ * NULL d_found, a NULL corpus with non-empty strings and n >= 2^32 (string indices are u32) are PIRE_GPU_EINVAL; a
+ * host-only handle gets PIRE_GPU_ENODEVICE.  Asynchronous on `stream`; re-entrant across streams on one handle (per-call
+ * scratch).  It costs about pire_gpu_count_batch_from plus a walk of the strings that have entries, and the writes of the
+ * entries (DESIGN.md 4).  Not covered, as in pire_gpu_count_batch_from: ordered batches (d_order) and line batches. */
+int pire_gpu_match_ends_batch_from(const pire_gpu_scanner* sc,
+                                   const uint8_t* d_corpus, const uint64_t* d_offsets, uint64_t fixed_len, uint64_t n,
+                                   uint32_t flags, const uint32_t* d_start, uint64_t* d_pos,
+                                   uint32_t* d_strings, uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity, uint64_t* d_found,
+                                   uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
+
 /* The step before the path for line-oriented input (samples/pigrep/pigrep.cpp:38-45 calls
  * std::getline and then Runner(sc).Begin().Run(line).End() per line).
  * pire_gpu_split_lines finds the lines of a newline-delimited text resident in HBM:

@@ -467,6 +467,83 @@ private:
     bool Ran;
 };
 
+// Where the matches BatchCounter counts end (pire_gpu_match_ends_batch_from): BatchCounter's shape, with the entries
+// (stream, end, regexp id) appended to the caller-owned device arrays d_strings / d_ends / d_ids (each may be null) of
+// `capacity` entries, ordered by stream within one Run() and in walk order within a stream, and their number ADDED to the
+// caller-owned device word *d_found.  The states are carried in d_state[0..n) and the bytes each stream has consumed in
+// d_pos[0..n) (both caller-owned; the caller zeroes *d_found and d_pos before the first call), so an end is the number of
+// bytes of that stream consumed when the state was entered, and chained calls do not synchronise.  End() is a launch of
+// its own over n empty strings.  After the stream is synchronised, *d_found is the number of entries (all of them, even
+// past capacity), the first min(*d_found, capacity) entries are the answer's first ones, and d_state / d_match_bits are
+// as BatchCounter's.
+//     BatchMatchEnds m(gsc, n, d_pos, d_strings, d_ends, d_ids, capacity, d_found, d_state);                    // Initialize()
+//     BatchMatchEnds m(gsc, BatchMatchEnds::From(d_start), n, d_pos, d_strings, d_ends, d_ids, capacity, d_found, d_state);
+//     m.Begin().Run(batch0).Run(batch1).End();
+class BatchMatchEnds {
+public:
+    using StartWords = BatchRunner::StartWords;
+    static StartWords From(const uint32_t* d_start) { return StartWords(d_start); }
+
+    BatchMatchEnds(const Scanner& sc, uint64_t n, uint64_t* d_pos, uint32_t* d_strings, uint64_t* d_ends, uint32_t* d_ids,
+                   uint64_t capacity, uint64_t* d_found, uint32_t* d_state, uint32_t* d_match_bits = nullptr, void* stream = nullptr)
+        : Sc(&sc), N(n), Start(nullptr), Pos(d_pos), Strings(d_strings), Ends(d_ends), Ids(d_ids), Capacity(capacity), Found(d_found),
+          State(d_state), Bits(d_match_bits), Stream(stream), Flags(0), Ran(false)
+    {
+        if (!d_found || (n != 0 && (!d_pos || !d_state)))
+            throw Error(PIRE_GPU_EINVAL, "BatchMatchEnds needs device words for the number of entries, the positions and the states");
+    }
+    // start.Words may be d_state: the states are then updated in place
+    BatchMatchEnds(const Scanner& sc, StartWords start, uint64_t n, uint64_t* d_pos, uint32_t* d_strings, uint64_t* d_ends,
+                   uint32_t* d_ids, uint64_t capacity, uint64_t* d_found, uint32_t* d_state, uint32_t* d_match_bits = nullptr,
+                   void* stream = nullptr)
+        : BatchMatchEnds(sc, n, d_pos, d_strings, d_ends, d_ids, capacity, d_found, d_state, d_match_bits, stream)
+    {
+        if (n != 0 && !start.Words)
+            throw Error(PIRE_GPU_EINVAL, "BatchMatchEnds::From needs device words");
+        Start = start.Words;
+    }
+
+    BatchMatchEnds& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }
+    BatchMatchEnds& Run(const Batch& b)
+    {
+        if (b.Count != N)
+            throw Error(PIRE_GPU_EINVAL, "BatchMatchEnds::Run needs a batch of n strings");
+        Launch(b, 0);
+        return *this;
+    }
+    BatchMatchEnds& End()
+    {
+        const Batch empty = {nullptr, nullptr, 0, N};
+        Launch(empty, PIRE_GPU_RUN_END);
+        return *this;
+    }
+
+private:
+    void Launch(const Batch& b, unsigned end)
+    {
+        Check(pire_gpu_match_ends_batch_from(Sc->Raw(), b.Corpus, b.Offsets, b.FixedLen, b.Count, Flags | end, Ran ? State : Start,
+                                             Pos, Strings, Ends, Ids, Capacity, Found, Bits, State, Stream),
+              "pire_gpu_match_ends_batch_from");
+        Flags = 0;
+        Ran = true;
+    }
+
+    const Scanner* Sc;
+    uint64_t N;
+    const uint32_t* Start;
+    uint64_t* Pos;
+    uint32_t* Strings;
+    uint64_t* Ends;
+    uint32_t* Ids;
+    uint64_t Capacity;
+    uint64_t* Found;
+    uint32_t* State;
+    uint32_t* Bits;
+    void* Stream;
+    unsigned Flags;
+    bool Ran;
+};
+
 // AcceptedRegexps for scanners with more than 32 regexps: rows of AcceptWords(sc) words, bit r of row i set iff
 // regexp r is accepted by the state string i stopped in (d_state_idx from BatchRunner::Launch).
 inline uint32_t AcceptWords(const Scanner& sc) { return pire_gpu_accept_words(sc.Raw()); }

@@ -38,7 +38,7 @@ SYMBOLS = [
     "pire_gpu_shard_bounds", "pire_gpu_sharded_words", "pire_gpu_comm_get_id", "pire_gpu_comm_create",
     "pire_gpu_comm_adopt", "pire_gpu_comm_destroy", "pire_gpu_comm_info", "pire_gpu_comm_wait", "pire_gpu_run_sharded", "pire_gpu_comm_gather_bits",
     "pire_gpu_run_string", "pire_gpu_run_batch_from", "pire_gpu_count_string", "pire_gpu_count_batch_from",
-    "pire_gpu_match_ends_string",
+    "pire_gpu_match_ends_string", "pire_gpu_match_ends_batch_from",
 ]
 
 
@@ -79,6 +79,8 @@ def _load():
     lib.pire_gpu_count_string.argtypes = [vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp]
     lib.pire_gpu_count_batch_from.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp]
     lib.pire_gpu_match_ends_string.argtypes = [vp, vp, C.c_uint64, C.c_uint32, vp, C.c_uint64, vp, vp, C.c_uint64, vp, vp, vp, vp]
+    lib.pire_gpu_match_ends_batch_from.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp, C.c_uint64, vp,
+                                                   vp, vp, vp]
     lib.pire_gpu_length_order.argtypes = [vp, C.c_uint64, vp, C.c_int, vp]
     lib.pire_gpu_run_batch_ordered.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, vp]
     lib.pire_gpu_split_lines.argtypes = [vp, C.c_uint64, vp, C.c_uint64, C.POINTER(C.c_uint64), C.c_int, vp]

@@ -505,6 +505,43 @@ int pire_gpu_count_batch_from(const pire_gpu_scanner* sc, const uint8_t* d_corpu
     return PIRE_GPU_OK;
 }
 
+int pire_gpu_match_ends_batch_from(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,
+                                   uint64_t fixed_len, uint64_t n, uint32_t flags, const uint32_t* d_start, uint64_t* d_pos,
+                                   uint32_t* d_strings, uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity, uint64_t* d_found,
+                                   uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream)
+{
+    int rc = CheckRunnable(sc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_match_ends_batch_from takes PIRE_GPU_RUN_BEGIN and PIRE_GPU_RUN_END only");
+    if (n == 0)
+        return PIRE_GPU_OK;
+    if (!d_found)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_match_ends_batch_from needs a device word for the number of entries");
+    if (!d_corpus && (d_offsets || fixed_len != 0))
+        return Fail(PIRE_GPU_EINVAL, "null corpus with non-empty strings");
+    if (n >= (1ull << 32))
+        return Fail(PIRE_GPU_EINVAL, "too many strings: string indices are u32");
+    CUDA_TRY(cudaSetDevice(sc->device));
+    ScanArgs a;
+    FillArgs(sc, &a, d_corpus, d_offsets, fixed_len, n, flags);
+    SetCounting(sc, &a, flags);
+    if (d_start)
+        SetStarts(sc, &a, d_start, flags);
+    a.match_bits = d_match_bits;
+    a.state_idx = d_state_idx;
+    a.uniform = IsUniform(d_corpus, d_offsets, fixed_len) ? 1 : 0;
+    a.pos = d_pos;
+    a.strings = d_strings;
+    a.ends = d_ends;
+    a.ids = d_ids;
+    a.ends_capacity = capacity;
+    a.found = reinterpret_cast<unsigned long long*>(d_found);
+    CUDA_TRY(LaunchMatchEndsBatch(a, sc->device, static_cast<cudaStream_t>(stream)));
+    return PIRE_GPU_OK;
+}
+
 uint32_t pire_gpu_accept_words(const pire_gpu_scanner* sc) { return sc ? sc->accept_words : 0; }
 
 int pire_gpu_accept_sets(const pire_gpu_scanner* sc, const uint32_t* d_state_idx, uint64_t n, uint32_t* d_accept_sets, void* stream)

@@ -89,6 +89,13 @@ struct ScanArgs {
     unsigned long long* found;   // one word, read and added to
     uint64_t ends_base;          // position of the text's first byte in the caller's numbering
     unsigned long long* string_sums; // scratch: each CTA's number of entries
+    // where the matches end in a batch of streams (pire_gpu_match_ends_batch_from): ends, ids, ends_capacity and found as
+    // above (ends_base 0), string i's entries in the slice [entry_first[i], entry_first[i + 1]), its positions from pos[i] on
+    uint32_t* strings;           // the string index of each entry, or null
+    uint64_t* pos;               // n words: each string's first position, advanced by its length; or null (all 0)
+    unsigned long long* entry_counts;      // scratch, n + 1: *found as the call found it, then each string's entries
+    const unsigned long long* entry_first; // scratch, n + 1: the inclusive sum of entry_counts
+    uint32_t* last_states;       // scratch, n: each string's state before EndMark, new numbering (0xFFFFFFFF: unknown start)
 };
 
 struct LaunchPlan {
@@ -138,6 +145,10 @@ cudaError_t LaunchPrefix(const ScanArgs& a, bool shortest, bool reverse, int dev
 // `from` (pire_gpu_count_batch_from) added to a.counts64 (n rows of u64), every string from a.starts[i] when a.starts is
 // given, its last state reported in a.match_bits / a.state_idx through a.fin
 cudaError_t LaunchCount(const ScanArgs& a, int device, cudaStream_t stream, bool from = false);
+// Every TakeAction of HalfFinalScanner on each string of a batch (MatchEndsBatchKernel): LaunchCount's walk with
+// `from`, string i's entries from index *a.found + (the entries of strings 0..i-1) on, placed by a scan over the strings;
+// then match bits, states and a.pos as LaunchCount's, and *a.found advanced by the call's total
+cudaError_t LaunchMatchEndsBatch(const ScanArgs& a, int device, cudaStream_t stream);
 // d_order <- string indices, longest half-octave length bucket first, corpus order inside a bucket (stable CUB radix sort).
 // stream-ordered scratch from the library's own per-device pool (see scan_kernels.cu)
 cudaError_t ScratchAlloc(void** out, size_t bytes, cudaStream_t stream);

@@ -711,6 +711,145 @@ class BatchCounter:
         return self.StateTensor().cpu().numpy().view(np.uint32)
 
 
+class BatchMatchEnds:
+    """Where the matches ``BatchCounter`` counts end (pire_gpu_match_ends_batch_from): one entry (stream, end, regexp id)
+    for every count, ordered by stream, then in walk order within a stream, where end is the number of bytes of that
+    stream consumed (over all ``Run()`` calls) when the final state was entered.  The entries go to device tensors of
+    ``capacity`` entries; ``FoundTensor()`` counts all of them, even past the capacity, whose entries are dropped (the
+    written ones are then the answer's first ``capacity``).  Every ``Run(batch)`` launches at once on the current stream,
+    string i of the batch being the next piece of stream i, and appends its entries; the states and the streams' byte
+    offsets are carried in device tensors, so rounds need no synchronise.  ``states`` (an int32 CUDA tensor of n
+    StateIndex values) resumes stream i from states[i] (not reported again), None = Initialize() (reported).
+    ``Begin()`` is folded into the next launch, ``End()`` is a launch of its own over n empty strings.
+    ``StringsTensor()``, ``EndsTensor()``, ``IdsTensor()``, ``FoundTensor()``, ``StateTensor()`` and ``PosTensor()`` do
+    not synchronise; ``Found()``, ``Strings()``, ``Ends()``, ``Ids()``, ``Matches()`` and ``States()`` do."""
+
+    def __init__(self, sc, n, capacity, states=None):
+        torch = _torch()
+        self.Sc = sc
+        self.n = int(n)
+        self.capacity = int(capacity)
+        dev = torch.device("cuda", sc.device)
+        if states is not None and (states.dtype != torch.int32 or not states.is_cuda or not states.is_contiguous()
+                                   or states.device != dev or states.numel() < self.n):
+            raise ValueError("states must be a contiguous int32 CUDA tensor of n states on the scanner's device")
+        self._start = states
+        self._states = torch.empty(self.n, dtype=torch.int32, device=dev)
+        self._bits = torch.empty((self.n + 31) // 32, dtype=torch.int32, device=dev)
+        self._pos = torch.zeros(self.n, dtype=torch.int64, device=dev)
+        self._strings = torch.empty(self.capacity, dtype=torch.int32, device=dev)
+        self._ends = torch.empty(self.capacity, dtype=torch.int64, device=dev)
+        self._ids = torch.empty(self.capacity, dtype=torch.int32, device=dev)
+        self._found = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._begin = False
+        self._ran = False          # a launch has written the states
+
+    def Begin(self):
+        if self._ran:
+            raise ValueError("Begin() must precede Run()")
+        self._begin = True
+        return self
+
+    def Run(self, batch):
+        if batch.trim:
+            raise ValueError("line batches have no per-string starts")
+        if batch.order is not None:
+            raise ValueError("BatchMatchEnds takes no length-ordered batch")
+        if batch.n != self.n:
+            raise ValueError("BatchMatchEnds.Run needs a batch of n = %d strings, got %d" % (self.n, batch.n))
+        if batch.device != self._states.device:
+            raise ValueError("the batch must be on the scanner's device")
+        self._launch(batch.corpus.data_ptr(), None if batch.offsets is None else batch.offsets.data_ptr(), batch.fixed_len, 0)
+        return self
+
+    def End(self):
+        self._launch(None, None, 0, N.RUN_END)
+        return self
+
+    def _launch(self, corpus, offsets, fixed_len, flags):
+        if self._begin:
+            flags |= N.RUN_BEGIN
+            self._begin = False
+        torch = _torch()
+        if self._ran:
+            start = self._states.data_ptr()
+        else:
+            start = None if self._start is None else self._start.data_ptr()
+        stream = torch.cuda.current_stream(self._states.device).cuda_stream
+        N.check(N.lib.pire_gpu_match_ends_batch_from(self.Sc._h, corpus, offsets, fixed_len, self.n, flags, start,
+                                                     self._pos.data_ptr(), self._strings.data_ptr(), self._ends.data_ptr(),
+                                                     self._ids.data_ptr(), self.capacity, self._found.data_ptr(),
+                                                     self._bits.data_ptr(), self._states.data_ptr(), stream),
+                "pire_gpu_match_ends_batch_from")
+        self._ran = True
+
+    def _ensure(self):
+        if not self._ran:
+            self._launch(None, None, 0, 0)      # nothing run yet: the start states (after Begin() if it was asked for)
+
+    # without a synchronise ------------------------------------------------------------
+    def StringsTensor(self):
+        """The device tensor of stream indices (int32 holding u32), ``capacity`` long."""
+        self._ensure()
+        return self._strings
+
+    def EndsTensor(self):
+        """The device tensor of ends (int64 holding u64), ``capacity`` long."""
+        self._ensure()
+        return self._ends
+
+    def IdsTensor(self):
+        """The device tensor of regexp ids (int32 holding u32), ``capacity`` long."""
+        self._ensure()
+        return self._ids
+
+    def FoundTensor(self):
+        """The device word (int64 holding u64) counting every entry, also those past the capacity."""
+        self._ensure()
+        return self._found
+
+    def StateTensor(self):
+        """The device tensor (int32, n) of the states reached, reference numbering: the ``states`` of a later
+        BatchCounter or BatchMatchEnds."""
+        self._ensure()
+        return self._states
+
+    def PosTensor(self):
+        """The device tensor (int64 holding u64, n) of the bytes each stream has consumed so far."""
+        self._ensure()
+        return self._pos
+
+    # synchronising --------------------------------------------------------------------
+    def Found(self):
+        """The number of entries, also those past the capacity."""
+        return int(self.FoundTensor().item())
+
+    def Strings(self):
+        """The first min(Found(), capacity) stream indices, as numpy u32."""
+        k = min(self.Found(), self.capacity)
+        return self._strings[:k].cpu().numpy().view(np.uint32)
+
+    def Ends(self):
+        """The first min(Found(), capacity) ends, as numpy u64."""
+        k = min(self.Found(), self.capacity)
+        return self._ends[:k].cpu().numpy().view(np.uint64)
+
+    def Ids(self):
+        """The first min(Found(), capacity) regexp ids, as numpy u32."""
+        k = min(self.Found(), self.capacity)
+        return self._ids[:k].cpu().numpy().view(np.uint32)
+
+    def Matches(self):
+        """numpy bool[n]: Final() of each stream's state."""
+        self._ensure()
+        words = self._bits.cpu().numpy().view(np.uint32)
+        return np.unpackbits(words.view(np.uint8), bitorder="little")[: self.n].astype(bool)
+
+    def States(self):
+        """StateIndex() of each stream's state (reference numbering); 0xFFFFFFFF for a start outside the scanner."""
+        return self.StateTensor().cpu().numpy().view(np.uint32)
+
+
 def Runner(sc, states=None):
     """Pire::Runner(sc) (run.h:388-389); with ``states`` Pire::Runner(sc, st) (run.h:391-392) for every string."""
     return RunHelper(sc, states)

@@ -262,5 +262,18 @@ assert full.Found() == part.Found() == total
 assert (part.Ends() == full.Ends()[: total // 2]).all() and (part.Ids() == full.Ids()[: total // 2]).all()
 assert np.bincount(full.Ids(), minlength=max(1, sc.RegexpsCount())).tolist() == [cnt.Result(r) for r in range(max(1, sc.RegexpsCount()))]
 print("ok match_ends_string", flush=True)
+# where the matches end in many streams (pire_gpu_match_ends_batch_from): the ragged batch above in its two rounds, into
+# a buffer too small for the answer, against BatchCounter on the same rounds and a call with room for all of it
+regs = max(1, sc.RegexpsCount())
+halves = [P.Batch.from_strings([s[:x] if k == 0 else s[x:] for s, x in zip(strings, cuts)]) for k in (0, 1)]
+c = P.BatchCounter(sc, len(strings)).Begin().Run(halves[0]).Run(halves[1]).End()
+total = int(c.Counts().sum().item())
+full = P.BatchMatchEnds(sc, len(strings), total).Begin().Run(halves[0]).Run(halves[1]).End()
+part = P.BatchMatchEnds(sc, len(strings), total // 2).Begin().Run(halves[0]).Run(halves[1]).End()
+assert full.Found() == part.Found() == total
+assert (part.Ends() == full.Ends()[: total // 2]).all() and (part.Strings() == full.Strings()[: total // 2]).all()
+key = full.Strings().astype(np.int64) * regs + full.Ids()
+assert (np.bincount(key, minlength=len(strings) * regs).reshape(-1, regs) == c.Counts().cpu().numpy()).all()
+print("ok match_ends_batch_from", flush=True)
 torch.cuda.synchronize()
 print("sanitize_run done, launches:", N.lib.pire_gpu_launch_count())
