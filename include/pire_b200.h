@@ -412,7 +412,10 @@ int pire_gpu_run_lines(const pire_gpu_scanner* sc, const uint8_t* d_text, const 
  * CSR batches are length-binned per chunk (pire_gpu_length_order).  Results are those of pire_gpu_run_batch on
  * the resident corpus.  Returns after everything has landed in the caller's arrays.
  * corpus_bytes = size of the corpus buffer; offsets (if any) must ascend and end within it, n * fixed_len
- * must fit in it (PIRE_GPU_EINVAL otherwise).
+ * must fit in it (PIRE_GPU_EINVAL otherwise).  A line batch (PIRE_GPU_RUN_LINES, the offsets of
+ * pire_gpu_split_lines for the text) needs the text up to offsets[n] - 1 only: a last line without '\n' has its
+ * separator one byte past the text, so corpus_bytes = the text's size is right with or without a final newline.
+ * Line batches are not length-binned; lines are scanned where they lie, as in pire_gpu_run_lines.
  * Concurrency: calls on one handle from several threads run concurrently, each with its own workspace
  * (streams, slots, staging); workspaces are kept with the handle and freed by pire_gpu_scanner_destroy. */
 int pire_gpu_run_batch_host(const pire_gpu_scanner* sc,

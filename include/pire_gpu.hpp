@@ -642,12 +642,14 @@ inline void HalfFinalCount(const Scanner& sc, const Batch& b, uint32_t* d_counts
 }
 
 // Host-buffer counterpart of `bool Pire::Runner(sc).Begin().Run(p, n).End()` for many
-// strings at once (CSR): fills `matched[i]`.
+// strings at once (CSR): fills `matched[i]`.  With PIRE_GPU_RUN_LINES the offsets are those of a text's lines
+// (std::getline), and the corpus is read up to offsets[n] - 1: a last line without '\n' ends at the text's end.
 inline void MatchesHost(const Scanner& sc, const uint8_t* corpus, const uint64_t* offsets, uint64_t n,
                         std::vector<bool>& matched, unsigned flags = PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END)
 {
     std::vector<uint32_t> bits((n + 31) / 32);
-    Check(pire_gpu_run_batch_host(sc.Raw(), corpus, n ? offsets[n] : 0, offsets, 0, n, flags, bits.data(), nullptr, nullptr),
+    const uint64_t bytes = n ? offsets[n] - ((flags & PIRE_GPU_RUN_LINES) ? 1 : 0) : 0;
+    Check(pire_gpu_run_batch_host(sc.Raw(), corpus, bytes, offsets, 0, n, flags, bits.data(), nullptr, nullptr),
           "pire_gpu_run_batch_host");
     matched.resize(n);
     for (uint64_t i = 0; i < n; ++i)

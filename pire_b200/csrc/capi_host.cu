@@ -15,7 +15,6 @@
 #include "capi_internal.hpp"
 
 #include <algorithm>
-#include <atomic>
 #include <cstdlib>
 #include <cstring>
 #include <functional>
@@ -60,7 +59,7 @@ public:
             src_ = src;
             bytes_ = bytes;
             pieces_ = (bytes + kPiece - 1) / kPiece;
-            next_.store(0);
+            next_ = 0;
             left_ = pieces_;
             ++generation_;
         }
@@ -71,16 +70,21 @@ public:
     }
 
 private:
+    // A piece is claimed under the lock, together with the buffers it belongs to: a helper still on its way out of
+    // the previous copy cannot take a piece number from one copy and the buffers or the count of the next, so every
+    // piece is counted off exactly once and Copy returns only when all of them have landed.
     void Drain()
     {
         constexpr size_t kPiece = 2u << 20;
-        for (;;) {
-            const size_t k = next_.fetch_add(1);
-            if (k >= pieces_)
-                return;
-            const size_t at = k * kPiece;
-            StageCopy(dst_ + at, src_ + at, std::min(kPiece, bytes_ - at));
-            std::lock_guard<std::mutex> lock(mu_);
+        std::unique_lock<std::mutex> lock(mu_);
+        while (next_ < pieces_) {
+            const size_t at = next_++ * kPiece;
+            uint8_t* dst = dst_ + at;
+            const uint8_t* src = src_ + at;
+            const size_t len = std::min(kPiece, bytes_ - at);
+            lock.unlock();
+            StageCopy(dst, src, len);
+            lock.lock();
             if (--left_ == 0)
                 done_.notify_all();
         }
@@ -106,8 +110,7 @@ private:
     uint64_t generation_ = 0;
     uint8_t* dst_ = nullptr;
     const uint8_t* src_ = nullptr;
-    size_t bytes_ = 0, pieces_ = 0, left_ = 0;
-    std::atomic<size_t> next_{0};
+    size_t bytes_ = 0, pieces_ = 0, next_ = 0, left_ = 0;
 };
 
 size_t EnvSize(const char* name, size_t fallback)
@@ -274,6 +277,7 @@ int RunStreamed(const pire_gpu_scanner* sc, HostWorkspace* ws, const Caller& c, 
     }
     const size_t chunk_bytes = EnvSize("PIRE_B200_HOST_CHUNK_MB", 64) << 20;
     const bool csr = c.offsets != nullptr;
+    const bool lines = csr && (flags & PIRE_GPU_RUN_LINES);
     const int outputs = (c.match_bits ? 1 : 0) + (c.accept_masks ? 1 : 0) + (c.state_idx ? 1 : 0);
 
     uint64_t first = 0;
@@ -286,7 +290,7 @@ int RunStreamed(const pire_gpu_scanner* sc, HostWorkspace* ws, const Caller& c, 
         }
         // this chunk: whole 32-string units, about chunk_bytes of corpus
         uint64_t count;
-        uint64_t byte_lo, byte_hi;
+        uint64_t byte_lo, byte_hi, copy_hi;
         if (csr) {
             byte_lo = c.offsets[first];
             uint64_t last = first;
@@ -295,15 +299,19 @@ int RunStreamed(const pire_gpu_scanner* sc, HostWorkspace* ws, const Caller& c, 
             } while (last < c.n && c.offsets[std::min<uint64_t>(c.n, last + 32)] - byte_lo <= chunk_bytes);
             count = last - first;
             byte_hi = c.offsets[last];
-            if (byte_hi < byte_lo || byte_hi > corpus_bytes)
+            // the batch's last line ends at a separator that may be the virtual one after the text
+            // (pire_gpu_split_lines); no kernel reads that byte, so the copy stops short of it
+            copy_hi = lines && last == c.n ? byte_hi - 1 : byte_hi;
+            if (byte_hi < byte_lo || copy_hi < byte_lo || copy_hi > corpus_bytes)
                 return Fail(PIRE_GPU_EINVAL, "offsets are not ascending or run past corpus_bytes");
         } else {
             const uint64_t per = c.fixed_len ? std::max<uint64_t>(32, chunk_bytes / c.fixed_len / 32 * 32) : c.n;
             count = std::min<uint64_t>(per, c.n - first);
             byte_lo = first * c.fixed_len;
             byte_hi = byte_lo + count * c.fixed_len;
+            copy_hi = byte_hi;
         }
-        const size_t bytes = (size_t) (byte_hi - byte_lo);
+        const size_t bytes = (size_t) (copy_hi - byte_lo);
         const size_t words = (size_t) ((count + 31) / 32);
         const size_t out_words = (c.match_bits ? words : 0) + (size_t) ((c.accept_masks ? 1 : 0) + (c.state_idx ? 1 : 0)) * count;
 
@@ -390,7 +398,10 @@ extern "C" int pire_gpu_run_batch_host(const pire_gpu_scanner* csc, const uint8_
     if (!corpus && corpus_bytes != 0)
         return Fail(PIRE_GPU_EINVAL, "null corpus with corpus_bytes != 0");
     if (offsets) {
-        if (offsets[n] > corpus_bytes || offsets[0] > offsets[n])
+        // a line batch needs the text up to its last separator, and a last line without '\n' has a virtual one at
+        // offsets[n] - 1 == the text's size
+        const uint64_t end = offsets[n] - ((flags & PIRE_GPU_RUN_LINES) ? 1 : 0);
+        if (end > corpus_bytes || offsets[0] > end)
             return Fail(PIRE_GPU_EINVAL, "offsets run past corpus_bytes");
     } else if (fixed_len != 0 && (corpus_bytes / fixed_len < n)) {
         return Fail(PIRE_GPU_EINVAL, "n * fixed_len exceeds corpus_bytes");

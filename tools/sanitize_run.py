@@ -12,7 +12,7 @@ import torch
 import pire_b200 as P
 from pire_b200 import _native as N
 from pire_b200 import workloads as W
-from refpire import Oracle
+from refpire import Oracle, csr
 
 dev = "cuda:0"
 
@@ -57,6 +57,17 @@ check(sc, orc, b, hc, ho, 0, 1500, "mixed binned")
 bits, masks, states = sc.run_batch_host(hc, offsets=ho, want_masks=True, want_states=True)
 f, m, s = orc.run(hc, ho)
 assert (np.unpackbits(bits.view(np.uint8), bitorder="little")[:1500] == f).all() and (states == s).all()
+# the lines of a text without a final newline, from a buffer of exactly its size: the last line's virtual separator
+# lies one byte past the text, and nothing may be read there
+text = b"\n".join(b"line %d hello  world" % i if i % 5 else b"" for i in range(3000)) + b"\nlast hello world"
+htext = np.frombuffer(text, np.uint8).copy()
+hl = np.concatenate([[0], np.flatnonzero(htext == 10) + 1, [len(text) + 1]]).astype(np.uint64)
+bits, _, states = sc.run_batch_host(htext, offsets=hl, flags=N.RUN_BEGIN | N.RUN_END | N.RUN_LINES, want_states=True)
+lines = text.split(b"\n")
+c, o = csr(lines)
+f, m, s = orc.run(c, o)
+assert (np.unpackbits(bits.view(np.uint8), bitorder="little")[:len(lines)] == f).all() and (states == s).all()
+assert int(f.sum()) > 100 and f[-1] == 1
 print("ok host entry")
 # odd shapes: empty strings, unaligned starts
 strings = [b"", b"x", b"hello world", b"\xd0\xbf" * 7 + b"HeLLo  World", b"a" * 33, b""] * 20
