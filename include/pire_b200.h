@@ -383,6 +383,53 @@ int pire_gpu_match_ends_batch_from(const pire_gpu_scanner* sc,
                                    uint32_t* d_strings, uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity, uint64_t* d_found,
                                    uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
 
+/* Where the matches whose ends the two calls above list start: the span of each match, for grep -o, highlighting or
+ * extracting a field.  Pire's own answer (run.h:312-342): LongestSuffix through a scanner built with Fsm::Reverse()
+ * ("consider using Fsm::Reverse() for using in this function"), walked leftwards from the match's end.
+ *   rsc     a plain Scanner image compiled from the same patterns with Fsm::Reverse() and without Surround(); for
+ *           several regexps the reversed scanners glued in the order of the forward HalfFinalScanner, so that regexp
+ *           ids agree.
+ *   Window  the text bytes the caller still holds, numbered as the entries' ends.  String form: [base, base + n_bytes)
+ *           of d_text.  Batch form (CSR or fixed length, as in pire_gpu_run_batch): string i covers
+ *           [d_pos[i] - len_i, d_pos[i]), d_pos being match_ends_batch_from's array as that call leaves it (one past
+ *           each string's last byte), so the same buffer is passed straight on; d_pos == NULL means len_i (ends are
+ *           offsets within each string).  d_strings == NULL means every entry belongs to string 0.
+ *   Entries indices [*d_first, min(*d_found, capacity)) of d_strings / d_ends / d_ids, as match_ends wrote them.  Both
+ *           words are read on the device, so this call can follow a match-ends call on the same stream with no
+ *           synchronise; d_first == NULL means 0.  A caller that chains chunks copies *d_found into d_first (8 bytes,
+ *           device to device) before each match-ends call.  An entry whose end lies outside its string's window, or
+ *           whose string is >= n, is not written: one entry array can be processed window by window.
+ *   Answer  d_starts[k]: the least s such that the reversed walk from end_k leftwards accepts over [s, end_k), where
+ *           "accepts" means id_k is in AcceptedRegexps(state) -- Final(state) when d_ids == NULL, which is exactly
+ *           LongestSuffix -- or PIRE_GPU_NO_START.  The walk steps BeginMark last when it reaches the window start and
+ *           PIRE_GPU_RUN_BEGIN says that is where the text begins.  An entry at the window's end under PIRE_GPU_RUN_END
+ *           is walked twice, without and with EndMark stepped first, and the longer answer is kept (a match-ends entry
+ *           does not record whether its match took the EndMark step); every other entry is walked without EndMark.  So
+ *           start_k is the leftmost start of a match of id_k ending at end_k, with BeginMark and EndMark only at the
+ *           text's real edges.  max_back > 0 bounds each walk to [max(window start, end_k - max_back), end_k); BeginMark
+ *           is then stepped only when that bound is the window start.
+ *   Open    d_open[k] (may be NULL) is 1 when a walk of entry k reached its lower bound in a state from which id_k
+ *           (with d_ids == NULL: a final state) can still be accepted and no BeginMark step settled it: bytes further
+ *           left could move the start left, so the caller may widen the window (or max_back) and call again.
+ *   flags   PIRE_GPU_RUN_BEGIN and/or PIRE_GPU_RUN_END; anything else (LINES included) is PIRE_GPU_EINVAL.
+ * Nothing outside the processed index range is written.  A NULL d_ends, d_found or d_starts and a NULL text with a
+ * non-empty window are PIRE_GPU_EINVAL; a host-only handle gets PIRE_GPU_ENODEVICE; n == 0 or capacity == 0 is a
+ * no-op.  Asynchronous on `stream`; re-entrant across streams on one handle (per-call scratch).  One entry per lane,
+ * each walk stopped as soon as id_k can no longer be accepted.  Worst case: a reversed regexp that never dies (the forward
+ * pattern has a .*-like prefix, e.g. hello\s+w.+d$ over printable text) walks back to the lower bound for every such
+ * entry, serially, at the speed of one lane; max_back is the bound for that case (DESIGN.md 4). */
+#define PIRE_GPU_NO_START 0xFFFFFFFFFFFFFFFFull
+int pire_gpu_match_starts_string(const pire_gpu_scanner* rsc, const uint8_t* d_text, uint64_t n_bytes, uint64_t base,
+                                 uint32_t flags, uint64_t max_back,
+                                 const uint64_t* d_ends, const uint32_t* d_ids,
+                                 const uint64_t* d_first, const uint64_t* d_found, uint64_t capacity,
+                                 uint64_t* d_starts, uint8_t* d_open, void* stream);
+int pire_gpu_match_starts_batch(const pire_gpu_scanner* rsc, const uint8_t* d_corpus, const uint64_t* d_offsets,
+                                uint64_t fixed_len, uint64_t n, const uint64_t* d_pos, uint32_t flags, uint64_t max_back,
+                                const uint32_t* d_strings, const uint64_t* d_ends, const uint32_t* d_ids,
+                                const uint64_t* d_first, const uint64_t* d_found, uint64_t capacity,
+                                uint64_t* d_starts, uint8_t* d_open, void* stream);
+
 /* The step before the path for line-oriented input (samples/pigrep/pigrep.cpp:38-45 calls
  * std::getline and then Runner(sc).Begin().Run(line).End() per line).
  * pire_gpu_split_lines finds the lines of a newline-delimited text resident in HBM:

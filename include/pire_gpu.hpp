@@ -348,6 +348,14 @@ private:
 //     StringMatchEnds m(gsc, d_ends, d_ids, capacity, d_found, d_state);                                  // Initialize()
 //     StringMatchEnds m(gsc, StringMatchEnds::From(d_start), d_ends, d_ids, capacity, d_found, d_state);  // resumed
 //     m.Begin().Run(d_a, n_a).Run(d_b, n_b).End();
+class StringMatchEnds;
+class BatchMatchEnds;
+void MatchStarts(const Scanner& rsc, const StringMatchEnds& ends, const uint8_t* d_window, uint64_t n_bytes, uint64_t base,
+                 uint64_t* d_starts, uint8_t* d_open = nullptr, bool begin = true, bool end = true, uint64_t max_back = 0,
+                 const uint64_t* d_first = nullptr);
+void MatchStarts(const Scanner& rsc, const BatchMatchEnds& ends, const Batch& window, uint64_t* d_starts, uint8_t* d_open = nullptr,
+                 bool begin = true, bool end = true, uint64_t max_back = 0, const uint64_t* d_first = nullptr);
+
 class StringMatchEnds {
 public:
     using StartWord = StringRunner::StartWord;
@@ -376,6 +384,8 @@ public:
     StringMatchEnds& End() { Launch(nullptr, 0, PIRE_GPU_RUN_END); return *this; }
 
 private:
+    friend void MatchStarts(const Scanner&, const StringMatchEnds&, const uint8_t*, uint64_t, uint64_t, uint64_t*, uint8_t*, bool,
+                            bool, uint64_t, const uint64_t*);
     void Launch(const uint8_t* d_text, uint64_t n, unsigned end)
     {
         Check(pire_gpu_match_ends_string(Sc->Raw(), d_text, n, Flags | end, Ran ? State : Start, Base, Ends, Ids, Capacity, Found,
@@ -519,6 +529,8 @@ public:
     }
 
 private:
+    friend void MatchStarts(const Scanner&, const BatchMatchEnds&, const Batch&, uint64_t*, uint8_t*, bool, bool, uint64_t,
+                            const uint64_t*);
     void Launch(const Batch& b, unsigned end)
     {
         Check(pire_gpu_match_ends_batch_from(Sc->Raw(), b.Corpus, b.Offsets, b.FixedLen, b.Count, Flags | end, Ran ? State : Start,
@@ -543,6 +555,33 @@ private:
     unsigned Flags;
     bool Ran;
 };
+
+// Where the matches of a StringMatchEnds / BatchMatchEnds start (pire_gpu_match_starts_string / _batch): Pire::LongestSuffix
+// through `rsc`, the same patterns built with Fsm::Reverse() and glued in the same order, walked leftwards from each
+// entry's end.  d_starts (and d_open, if given) get one word per entry of the ends' buffers, for entries
+// [*d_first, min(*d_found, capacity)); entries whose end lies outside the window are not written.  String form: the
+// window holds the text bytes at positions [base, base + n_bytes).  Batch form: the window is the batch of the ends'
+// last round (string i ends where the ends' d_pos says).  begin: the window starts where the text begins; end: the
+// ends' run took End().  On the ends' stream, with no synchronise.
+//     StringMatchEnds m(gsc, d_ends, d_ids, cap, d_found, d_state);
+//     m.Begin().Run(d_text, n).End();
+//     MatchStarts(rsc, m, d_text, n, 0, d_starts);
+inline void MatchStarts(const Scanner& rsc, const StringMatchEnds& ends, const uint8_t* d_window, uint64_t n_bytes, uint64_t base,
+                        uint64_t* d_starts, uint8_t* d_open, bool begin, bool end, uint64_t max_back, const uint64_t* d_first)
+{
+    Check(pire_gpu_match_starts_string(rsc.Raw(), d_window, n_bytes, base, (begin ? PIRE_GPU_RUN_BEGIN : 0u) | (end ? PIRE_GPU_RUN_END : 0u),
+                                       max_back, ends.Ends, ends.Ids, d_first, ends.Found, ends.Capacity, d_starts, d_open, ends.Stream),
+          "pire_gpu_match_starts_string");
+}
+
+inline void MatchStarts(const Scanner& rsc, const BatchMatchEnds& ends, const Batch& window, uint64_t* d_starts, uint8_t* d_open,
+                        bool begin, bool end, uint64_t max_back, const uint64_t* d_first)
+{
+    Check(pire_gpu_match_starts_batch(rsc.Raw(), window.Corpus, window.Offsets, window.FixedLen, window.Count, ends.Pos,
+                                      (begin ? PIRE_GPU_RUN_BEGIN : 0u) | (end ? PIRE_GPU_RUN_END : 0u), max_back, ends.Strings,
+                                      ends.Ends, ends.Ids, d_first, ends.Found, ends.Capacity, d_starts, d_open, ends.Stream),
+          "pire_gpu_match_starts_batch");
+}
 
 // AcceptedRegexps for scanners with more than 32 regexps: rows of AcceptWords(sc) words, bit r of row i set iff
 // regexp r is accepted by the state string i stopped in (d_state_idx from BatchRunner::Launch).

@@ -50,6 +50,7 @@ void DeviceTables::Free()
     cudaFree(weights);
     cudaFree(accept_wide);
     cudaFree(new_of_old);
+    cudaFree(live);
     *this = DeviceTables();
 }
 
@@ -146,6 +147,9 @@ int Upload(pire_gpu_scanner* sc)
         CUDA_TRY(cudaMalloc(&d.accept_wide, wide.size() * 4));
         CUDA_TRY(cudaMemcpy(d.accept_wide, wide.data(), wide.size() * 4, cudaMemcpyHostToDevice));
     }
+    CUDA_TRY(cudaMalloc(&d.live, t.live.size() * 4 + 4));
+    if (!t.live.empty())
+        CUDA_TRY(cudaMemcpy(d.live, t.live.data(), t.live.size() * 4, cudaMemcpyHostToDevice));
     // tuning renumbers the states: the map is rebuilt with the other tables
     CUDA_TRY(cudaMalloc(&d.new_of_old, t.new_of_old.size() * 4 + 4));
     if (!t.new_of_old.empty())
@@ -777,6 +781,74 @@ int pire_gpu_match_ends_string(const pire_gpu_scanner* sc, const uint8_t* d_text
     a.ends_base = base;
     CUDA_TRY(LaunchMatchEndsString(a, sc->device, static_cast<cudaStream_t>(stream)));
     return PIRE_GPU_OK;
+}
+
+// Both match-starts entry points: the string form is a batch of one string whose window ends at base + n_bytes.
+static int MatchStarts(const pire_gpu_scanner* rsc, const uint8_t* d_corpus, const uint64_t* d_offsets, uint64_t fixed_len,
+                       uint64_t n, const uint64_t* d_pos, uint64_t base, uint32_t flags, uint64_t max_back,
+                       const uint32_t* d_strings, const uint64_t* d_ends, const uint32_t* d_ids, const uint64_t* d_first,
+                       const uint64_t* d_found, uint64_t capacity, uint64_t* d_starts, uint8_t* d_open, void* stream)
+{
+    int rc = CheckRunnable(rsc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END))
+        return Fail(PIRE_GPU_EINVAL, "the match-starts calls take PIRE_GPU_RUN_BEGIN and PIRE_GPU_RUN_END only");
+    if (!d_ends || !d_found || !d_starts)
+        return Fail(PIRE_GPU_EINVAL, "the match-starts calls need d_ends, d_found and d_starts");
+    if (!d_corpus && (d_offsets || fixed_len != 0))
+        return Fail(PIRE_GPU_EINVAL, "null text with a non-empty window");
+    if (n == 0 || capacity == 0)
+        return PIRE_GPU_OK;
+    if (n >= (1ull << 32))
+        return Fail(PIRE_GPU_EINVAL, "too many strings: string indices are u32");
+    CUDA_TRY(cudaSetDevice(rsc->device));
+    ScanArgs a;
+    FillArgs(rsc, &a, d_corpus, d_offsets, fixed_len, n, 0);
+    a.flags = rsc->dev.flags;
+    a.fin = rsc->dev.fin[0];                      // AcceptedRegexps of the state itself
+    a.acc_begin = rsc->dev.acc_begin;
+    a.acc_ids = rsc->dev.acc_ids;
+    a.first_final_hot = rsc->tab.first_final_hot;
+    a.initial = rsc->tab.initial;
+    a.begin_class = rsc->tab.begin_class;
+    a.end_class = rsc->tab.end_class;
+    a.with_begin = (flags & PIRE_GPU_RUN_BEGIN) ? 1 : 0;
+    a.with_end = (flags & PIRE_GPU_RUN_END) ? 1 : 0;
+    a.live = rsc->dev.live;
+    a.live_words = rsc->tab.live_words;
+    a.window_end = d_pos;
+    a.ends_base = base;
+    a.max_back = max_back;
+    a.entry_strings = d_strings;
+    a.entry_ends = d_ends;
+    a.entry_ids = d_ids;
+    a.entries_first = reinterpret_cast<const unsigned long long*>(d_first);
+    a.entries_found = reinterpret_cast<const unsigned long long*>(d_found);
+    a.ends_capacity = capacity;
+    a.match_starts = d_starts;
+    a.match_open = d_open;
+    CUDA_TRY(LaunchMatchStarts(a, rsc->device, static_cast<cudaStream_t>(stream)));
+    return PIRE_GPU_OK;
+}
+
+int pire_gpu_match_starts_string(const pire_gpu_scanner* rsc, const uint8_t* d_text, uint64_t n_bytes, uint64_t base,
+                                 uint32_t flags, uint64_t max_back, const uint64_t* d_ends, const uint32_t* d_ids,
+                                 const uint64_t* d_first, const uint64_t* d_found, uint64_t capacity, uint64_t* d_starts,
+                                 uint8_t* d_open, void* stream)
+{
+    return MatchStarts(rsc, d_text, nullptr, n_bytes, 1, nullptr, base, flags, max_back, nullptr, d_ends, d_ids, d_first, d_found,
+                       capacity, d_starts, d_open, stream);
+}
+
+int pire_gpu_match_starts_batch(const pire_gpu_scanner* rsc, const uint8_t* d_corpus, const uint64_t* d_offsets,
+                                uint64_t fixed_len, uint64_t n, const uint64_t* d_pos, uint32_t flags, uint64_t max_back,
+                                const uint32_t* d_strings, const uint64_t* d_ends, const uint32_t* d_ids,
+                                const uint64_t* d_first, const uint64_t* d_found, uint64_t capacity,
+                                uint64_t* d_starts, uint8_t* d_open, void* stream)
+{
+    return MatchStarts(rsc, d_corpus, d_offsets, fixed_len, n, d_pos, 0, flags, max_back, d_strings, d_ends, d_ids, d_first,
+                       d_found, capacity, d_starts, d_open, stream);
 }
 
 int pire_gpu_scanner_tune(pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,

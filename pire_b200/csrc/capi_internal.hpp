@@ -41,6 +41,7 @@ struct DeviceTables {
     uint64_t* weights = nullptr;
     uint32_t* accept_wide = nullptr;     // [states x accept_words], reference numbering: AcceptedRegexps as a bit set
     uint32_t* new_of_old = nullptr;      // [states]: reference numbering -> new (start states given by the caller)
+    uint32_t* live = nullptr;            // ScanTables::live
     size_t full_bytes = 0;
 
     void Free();

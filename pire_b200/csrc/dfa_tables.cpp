@@ -244,6 +244,46 @@ void BuildScanTables(const Dfa& dfa, const std::vector<uint32_t>& hot_order, uin
         }
     }
 
+    // The ids still acceptable from each state: a fixpoint over the transitions, propagated backwards from the final
+    // states' accept lists with a worklist over the predecessors.
+    t.live_words = (regs + 31) / 32;
+    t.live.assign((size_t) dfa.states * t.live_words, 0);
+    {
+        const uint32_t W = t.live_words;
+        std::vector<uint32_t> pred_begin((size_t) dfa.states + 1, 0), preds((size_t) dfa.states * dfa.letters);
+        for (uint32_t ns = 0; ns < dfa.states; ++ns)
+            for (uint32_t c = 0; c < dfa.letters; ++c)
+                ++pred_begin[(t.wide ? t.full32[(size_t) ns * dfa.letters + c] : t.full16[(size_t) ns * dfa.letters + c]) + 1];
+        for (uint32_t ns = 0; ns < dfa.states; ++ns)
+            pred_begin[ns + 1] += pred_begin[ns];
+        std::vector<uint32_t> fill(pred_begin.begin(), pred_begin.end() - 1);
+        for (uint32_t ns = 0; ns < dfa.states; ++ns)
+            for (uint32_t c = 0; c < dfa.letters; ++c)
+                preds[fill[t.wide ? t.full32[(size_t) ns * dfa.letters + c] : t.full16[(size_t) ns * dfa.letters + c]]++] = ns;
+        std::vector<uint32_t> work;
+        for (uint32_t ns = 0; ns < dfa.states; ++ns) {
+            for (uint32_t k = t.acc_begin_new[ns]; k < t.acc_begin_new[ns + 1]; ++k)
+                t.live[(size_t) ns * W + t.acc_ids_new[k] / 32] |= 1u << (t.acc_ids_new[k] % 32);
+            work.push_back(ns);
+        }
+        while (!work.empty()) {
+            const uint32_t s = work.back();
+            work.pop_back();
+            const uint32_t* from = &t.live[(size_t) s * W];
+            for (uint32_t k = pred_begin[s]; k < pred_begin[s + 1]; ++k) {
+                uint32_t* to = &t.live[(size_t) preds[k] * W];
+                bool grew = false;
+                for (uint32_t w = 0; w < W; ++w)
+                    if (from[w] & ~to[w]) {
+                        to[w] |= from[w];
+                        grew = true;
+                    }
+                if (grew)
+                    work.push_back(preds[k]);
+            }
+        }
+    }
+
     t.start[0] = t.new_of_old[dfa.initial];                              // Initialize(), multi.h:161
     t.start[1] = t.new_of_old[dfa.Next(dfa.initial, kBeginMark)];        // Begin(), run.h:375
 }

@@ -83,6 +83,11 @@ struct ScanTables {
     // listed more than 15 times for one state); the kernel then walks the lists.
     uint32_t count_words = 0;
     std::vector<uint64_t> weights;
+    // Match starts (pire_gpu_match_starts_*): live[s * live_words + id / 32] bit id % 32 is set when some continuation
+    // from s (bytes and marks) reaches a final state that lists regexp id -- s itself included.  A reverse walk for id
+    // stops in a state without the bit: nothing further left can change its answer.
+    uint32_t live_words = 1;                 // ceil(max(1, regexps) / 32)
+    std::vector<uint32_t> live;              // [states * live_words], new numbering
 
     // Lane-private rows (kernel variant PRIV): the first priv_rows-1 hot ids, plus a sink
     // row (id priv_rows-1) that absorbs every transition into a non-private state.  Only

@@ -2347,6 +2347,7 @@ struct PrefixLane {
     uint32_t consumed;      // bytes walked so far
     uint32_t pos;           // answer so far, kNoPrefix = none
     bool stop;
+    static constexpr bool kAnyFinal = true;     // every final state counts (not one regexp's)
 };
 constexpr uint32_t kNoPrefix = 0xFFFFFFFFu;
 
@@ -2389,9 +2390,12 @@ __device__ __forceinline__ void PrefixCheck(const ScanArgs& a, uint32_t H, const
         l.stop = true;
 }
 
-template <bool kShortest, bool kReverse>
+// Whether hot id h (or H) counts in the branch-free replay of PrefixChunk16.
+__device__ __forceinline__ bool HotAccepts(const ScanArgs& a, uint32_t h, const PrefixLane&) { return h >= a.first_final_hot; }
+
+template <bool kShortest, bool kReverse, class Lane = PrefixLane>
 __device__ __forceinline__ void PrefixChunk16(const ScanArgs& a, const Tables& t, const uint8_t* hot_flags, LaneState& s, uint4 v,
-                                              PrefixLane& l)
+                                              Lane& l)
 {
     const uint32_t before = s.g;
     uint32_t g = before, top = 0, low = 0xffffffffu;
@@ -2412,7 +2416,7 @@ __device__ __forceinline__ void PrefixChunk16(const ScanArgs& a, const Tables& t
         l.consumed += 16;
         return;
     }
-    if (!kShortest && low >= a.first_final_hot && top != t.H) {
+    if (!kShortest && Lane::kAnyFinal && low >= a.first_final_hot && top != t.H) {
         // sixteen steps through final hot states (a lane behind an unanchored match sits in such states for the rest of
         // its string): the longest prefix so far ends with this chunk, no second pass needed
         s.g = g;
@@ -2435,7 +2439,7 @@ __device__ __forceinline__ void PrefixChunk16(const ScanArgs& a, const Tables& t
 #pragma unroll
             for (int b = 0; b < 4; ++b) {
                 FastStep<false, false>(t, h, word, 0x5540 + (kReverse ? 3 - b : b));
-                const bool final = h >= a.first_final_hot;
+                const bool final = HotAccepts(a, h, l);
                 if (kShortest)
                     mark = final && mark == 0 ? (uint32_t) (4 * w + b + 1) : mark;
                 else
@@ -2773,6 +2777,254 @@ __global__ void __maxnreg__(48) PrefixUniformKernel(const __grid_constant__ Scan
                     l.pos = ulen;
             }
             a.prefix_len[i] = l.pos;
+        }
+    }
+}
+
+// ---------------------------------------------------------------- where the matches start
+//
+// The leftmost start of a match that ends at a given position (pire_gpu_match_starts_*): Pire::LongestSuffix
+// (run.h:316-342) through a scanner built with Fsm::Reverse(), walked from the entry's end leftwards, one entry per lane.
+// The walk is the suffix scan's (PrefixChunk16 over 16-byte chunks of a per-lane cp.async ring, edge bytes byte by
+// byte); what differs is the lane: positions are 64-bit, "accepted" means the entry's regexp is in the state's accept
+// list (the bit of the hot state's mask for ids < 32, the list itself above), and the lane stops as soon as its state can
+// no longer reach a state accepting that regexp (ScanTables::live) -- on Dead() alone, a glued reversed scanner would
+// keep every entry walking as long as its longest-living sibling regexp.  Noticing that late changes nothing (such a
+// state only leads to such states), so it is looked at once per ring round.  Entries come in text order, so the lanes
+// of a warp read overlapping bytes; warps of a persistent grid take groups of 32 consecutive entries from a counter, so
+// that a few long walks hold up one warp and not a whole CTA's share.
+constexpr uint32_t kAnyRegexp = 0xFFFFFFFFu;
+constexpr uint64_t kNoStart = ~0ull;
+constexpr uint32_t kStartsHotLiveWords = 16;       // live rows up to this many words are staged in shared memory
+
+struct StartsLane {
+    uint64_t consumed;          // bytes walked so far
+    uint64_t pos;               // longest accepted suffix so far, kNoStart = none
+    bool stop;
+    uint32_t id;                // the entry's regexp, kAnyRegexp = Final()
+    const uint32_t* hot_mask;   // shared, H + 1 words: accept mask (ids < 32) of each final hot state, 0 for the rest
+    const uint32_t* hot_live;   // shared: the hot states' rows of ScanArgs::live, or null (read from global memory)
+    static constexpr bool kAnyFinal = false;
+};
+
+__device__ __forceinline__ bool AcceptsId(const ScanArgs& a, uint32_t state, uint32_t id)
+{
+    for (uint32_t k = __ldg(a.acc_begin + state), e = __ldg(a.acc_begin + state + 1); k < e; ++k)
+        if (__ldg(a.acc_ids + k) == id)
+            return true;
+    return false;
+}
+
+__device__ __forceinline__ bool HotAccepts(const ScanArgs& a, uint32_t h, const StartsLane& l)
+{
+    if (h < a.first_final_hot || h >= a.hot)
+        return false;
+    if (l.id < 32 || l.id == kAnyRegexp)
+        return l.id == kAnyRegexp || ((l.hot_mask[h] >> l.id) & 1u);
+    return AcceptsId(a, h, l.id);
+}
+
+// id_k in AcceptedRegexps(state) (Final(state) without an id)
+__device__ __forceinline__ bool StartsAccepts(const ScanArgs& a, uint32_t H, const uint8_t* hot_flags, uint32_t state,
+                                              const StartsLane& l)
+{
+    const uint32_t fl = state < H ? hot_flags[state] : __ldg(a.flags + state);
+    if (!(fl & 1u))
+        return false;
+    if (l.id == kAnyRegexp)
+        return true;
+    if (l.id < 32)
+        return ((state < H ? l.hot_mask[state] : __ldg(&a.fin[state].mask)) >> l.id) & 1u;
+    return AcceptsId(a, state, l.id);
+}
+
+// id_k can still be accepted from `state` (not Dead() without an id)
+__device__ __forceinline__ bool StartsLive(const ScanArgs& a, uint32_t H, const uint8_t* hot_flags, uint32_t state,
+                                           const StartsLane& l)
+{
+    if (l.id == kAnyRegexp)
+        return !((state < H ? hot_flags[state] : __ldg(a.flags + state)) & 2u);
+    const size_t at = (size_t) state * a.live_words + l.id / 32;
+    return ((state < H && l.hot_live ? l.hot_live[at] : __ldg(a.live + at)) >> (l.id % 32)) & 1u;
+}
+
+template <bool kShortest>
+__device__ __forceinline__ void PrefixCheck(const ScanArgs& a, uint32_t H, const uint8_t* hot_flags, uint32_t state, StartsLane& l)
+{
+    if (StartsAccepts(a, H, hot_flags, state, l))
+        l.pos = l.consumed;
+    if (!StartsLive(a, H, hot_flags, state, l))
+        l.stop = true;
+}
+
+__global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) MatchStartsKernel(const __grid_constant__ ScanArgs a)
+{
+    uint8_t* const smem = pire_b200_smem;
+    SharedView sv = CarveShared(smem, a.hot);
+    StageTables(a, sv, a.hot8, a.hot);
+    uint8_t* const hot_flags = sv.stage + kStageBytes;                       // H + 1 bytes behind the staging ring
+    uint32_t* const hot_mask = reinterpret_cast<uint32_t*>(hot_flags + 272); // H + 1 words
+    uint32_t* const hot_live = a.live_words <= kStartsHotLiveWords ? hot_mask + 256 : nullptr;
+    for (uint32_t i = threadIdx.x; i <= a.hot; i += blockDim.x) {
+        const uint32_t fl = i < a.hot ? a.flags[i] : 0;
+        hot_flags[i] = fl;
+        hot_mask[i] = (fl & 1u) ? a.fin[i].mask : 0;
+    }
+    if (hot_live)
+        for (uint32_t i = threadIdx.x; i < a.hot * a.live_words; i += blockDim.x)
+            hot_live[i] = a.live[i];
+    __syncthreads();
+
+    Tables t;
+    t.hot = sv.hot;
+    t.base = SmemAddr(sv.hot);
+    t.cls = sv.cls;
+    t.full = a.full;
+    t.H = a.hot;
+    t.letters = a.letters;
+    t.wide = a.wide;
+    t.m0 = 0;
+
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t stage = SmemAddr(sv.stage) + (((threadIdx.x >> 5) * kStageSlots) * 32 + lane) * 16;
+    const uintptr_t buf_lo = reinterpret_cast<uintptr_t>(a.corpus);
+    const uintptr_t buf_hi = buf_lo + (a.offsets ? a.offsets[a.n] : a.n * a.fixed_len);
+    const uint64_t first = a.entries_first ? *a.entries_first : 0;
+    const uint64_t found = *a.entries_found;
+    const uint64_t last = found < a.ends_capacity ? found : a.ends_capacity;
+    if (first >= last)
+        return;
+
+    for (;;) {
+        unsigned long long group = 0;
+        if (lane == 0)
+            group = atomicAdd(a.group_counter, 1ull);
+        group = __shfl_sync(0xffffffffu, group, 0);
+        if (group * 32 >= last - first)
+            break;
+        const uint64_t k = first + group * 32 + lane;
+        bool valid = k < last;
+        uint64_t end = 0, wstart = 0, wend = 0;
+        const uint8_t* wbase = a.corpus;
+        uint32_t id = kAnyRegexp;
+        if (valid) {
+            const uint32_t si = a.entry_strings ? a.entry_strings[k] : 0;
+            end = a.entry_ends[k];
+            valid = si < a.n;
+            if (valid) {
+                uint64_t b, e;
+                if (a.offsets) {
+                    b = a.offsets[si];
+                    e = a.offsets[si + 1];
+                    e = e < b ? b : e;
+                } else {
+                    b = (uint64_t) si * a.fixed_len;
+                    e = b + a.fixed_len;
+                }
+                wend = a.window_end ? a.window_end[si] : a.ends_base + (e - b);
+                wstart = wend - (e - b);
+                valid = wend >= e - b && end >= wstart && end <= wend;    // entries outside the window are not ours
+                wbase = a.corpus + b;
+                if (a.entry_ids)
+                    id = a.entry_ids[k];
+            }
+        }
+        const uint64_t lower = valid && a.max_back && end - wstart > a.max_back ? end - a.max_back : wstart;
+        const bool begin_here = a.with_begin && lower == wstart;
+        // an entry at the window's end under END: its match may have taken the EndMark step or not, the longer wins
+        const int passes = !valid ? 0 : (a.with_end && end == wend) ? 2 : 1;
+        uint64_t best = kNoStart;
+        bool open = false;
+        for (int pass = 0; __any_sync(0xffffffffu, pass < passes); ++pass) {
+            StartsLane l;
+            l.consumed = 0;
+            l.pos = kNoStart;
+            l.stop = pass >= passes;
+            l.id = id;
+            l.hot_mask = hot_mask;
+            l.hot_live = hot_live;
+            uint32_t full = pass == 1 ? FullNext(t, a.initial, a.end_class) : a.initial;
+            if (!l.stop)
+                PrefixCheck<false>(a, t.H, hot_flags, full, l);
+            const uint8_t* const lo = wbase + (lower - wstart);
+            const uint8_t* p = l.stop ? lo : wbase + (end - wstart);         // one past the next byte
+            // edge bytes up to a 16-byte boundary
+            {
+                const uint32_t misalign = (uint32_t) (reinterpret_cast<uintptr_t>(p) & 15);
+                const uint64_t len = (uint64_t) (p - lo);
+                if (len != 0 && misalign != 0) {
+                    const uint32_t nedge = len < misalign ? (uint32_t) len : misalign;
+                    const uint8_t* chunk = p - misalign;
+                    const bool whole = reinterpret_cast<uintptr_t>(chunk) >= buf_lo && reinterpret_cast<uintptr_t>(chunk) + 16 <= buf_hi;
+                    EdgeBytesDown eb(whole ? LoadEdge16(chunk) : make_uint4(0, 0, 0, 0), misalign - 1);
+                    for (uint32_t j = 0; j < nedge && !l.stop; ++j) {
+                        full = SlowStep(t, full, whole ? eb.Next() : (uint32_t) p[-1 - (int) j]);
+                        ++l.consumed;
+                        PrefixCheck<false>(a, t.H, hot_flags, full, l);
+                    }
+                    p -= nedge;
+                }
+            }
+            LaneState s;
+            SetFull(t, s, full);
+            // body: whole 16-byte chunks, chunk c at p - 16(c+1)
+            const uint64_t chunks = l.stop ? 0 : (uint64_t) (p - lo) >> 4;
+#pragma unroll
+            for (int j = 0; j < kStageSlots; ++j) {
+                if ((uint64_t) j < chunks)
+                    CopyAsync16(stage + j * 512, p - 16 * (j + 1));
+                CopyAsyncCommit();
+            }
+            for (uint64_t c = 0; __any_sync(0xffffffffu, c < chunks && !l.stop); c += kStageSlots) {
+#pragma unroll
+                for (int j = 0; j < kStageSlots; ++j) {
+                    CopyAsyncWait<kStageSlots - 1>();
+                    const uint4 v = LoadShared16(stage + j * 512);
+                    const bool had = c + j < chunks && !l.stop;
+                    if (c + kStageSlots + j < chunks && !l.stop)
+                        CopyAsync16(stage + j * 512, p - 16 * (c + kStageSlots + j + 1));
+                    CopyAsyncCommit();
+                    if (had)
+                        PrefixChunk16<false, true>(a, t, hot_flags, s, v, l);
+                }
+                if (!l.stop && !StartsLive(a, t.H, hot_flags, FullState(t, s), l))
+                    l.stop = true;
+            }
+            CopyAsyncWait<0>();
+            full = FullState(t, s);
+            // edge bytes on the far side: fewer than 16, p - 16 * chunks is on a 16-byte boundary
+            if (!l.stop) {
+                p -= 16 * chunks;
+                const uint32_t nfar = (uint32_t) (p - lo);
+                if (nfar != 0) {
+                    const uint8_t* chunk = p - 16;
+                    const bool whole = reinterpret_cast<uintptr_t>(chunk) >= buf_lo && reinterpret_cast<uintptr_t>(chunk) + 16 <= buf_hi;
+                    EdgeBytesDown eb(whole ? LoadEdge16(chunk) : make_uint4(0, 0, 0, 0), 15);
+                    for (uint32_t j = 0; j < nfar && !l.stop; ++j) {
+                        full = SlowStep(t, full, whole ? eb.Next() : (uint32_t) p[-1 - (int) j]);
+                        ++l.consumed;
+                        PrefixCheck<false>(a, t.H, hot_flags, full, l);
+                    }
+                }
+            }
+            if (pass < passes) {
+                // a lane that has not stopped walked every byte down to `lower`
+                if (!l.stop) {
+                    if (begin_here) {
+                        if (StartsAccepts(a, t.H, hot_flags, FullNext(t, full, a.begin_class), l))   // run.h:336-340
+                            l.pos = l.consumed;
+                    } else if (StartsLive(a, t.H, hot_flags, full, l)) {
+                        open = true;
+                    }
+                }
+                if (l.pos != kNoStart && (best == kNoStart || l.pos > best))
+                    best = l.pos;
+            }
+        }
+        if (valid) {
+            a.match_starts[k] = best == kNoStart ? kNoStart : end - best;
+            if (a.match_open)
+                a.match_open[k] = open ? 1 : 0;
         }
     }
 }
@@ -4342,6 +4594,36 @@ __global__ void __launch_bounds__(256) LengthKeysKernel(const uint64_t* __restri
 // that keeps up to 64 MiB cached.  The device's default pool returns everything to the driver at each
 // synchronisation, after which the next 4-byte counter allocation costs a 10-40 ms mapping stall -- seen as
 // one slow step in twenty on the length-binned path.
+// A persistent grid of the generic kernel's shape; behind the staging ring: the hot states' flag bytes (272), accept
+// masks (256 words) and, up to kStartsHotLiveWords words a row, their live rows.
+cudaError_t LaunchMatchStarts(const ScanArgs& a, int device, cudaStream_t stream)
+{
+    const void* fn = reinterpret_cast<const void*>(&MatchStartsKernel);
+    int optin = 0, sms = 0;
+    cudaError_t err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+    if (err == cudaSuccess)
+        err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err == cudaSuccess)
+        err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+    if (err != cudaSuccess)
+        return err;
+    const size_t shared = GenericSharedBytes(a.hot) + 272 + 256 * 4
+                          + (a.live_words <= kStartsHotLiveWords ? (size_t) a.hot * a.live_words * 4 : 0);
+    ScanArgs walk = a;
+    err = ScratchAlloc(reinterpret_cast<void**>(&walk.group_counter), 8, stream);
+    if (err != cudaSuccess)
+        return err;
+    err = cudaMemsetAsync(walk.group_counter, 0, 8, stream);
+    if (err == cudaSuccess) {
+        void* args[] = {&walk};
+        err = cudaLaunchKernel(fn, dim3(sms * kGenericBlocksPerSM), dim3(kBlock), args, shared, stream);
+        if (err == cudaSuccess)
+            g_launches.fetch_add(1, std::memory_order_relaxed);
+    }
+    cudaFreeAsync(walk.group_counter, stream);
+    return err;
+}
+
 cudaError_t ScratchAlloc(void** out, size_t bytes, cudaStream_t stream)
 {
     static std::mutex mu;

@@ -96,6 +96,23 @@ struct ScanArgs {
     unsigned long long* entry_counts;      // scratch, n + 1: *found as the call found it, then each string's entries
     const unsigned long long* entry_first; // scratch, n + 1: the inclusive sum of entry_counts
     uint32_t* last_states;       // scratch, n: each string's state before EndMark, new numbering (0xFFFFFFFF: unknown start)
+    // where the matches start (pire_gpu_match_starts_*): entries [*entries_first, min(*entries_found, ends_capacity)) of
+    // entry_strings / entry_ends / entry_ids; string i's window is [w - len_i, w) with w = window_end[i], or ends_base +
+    // len_i when that is null.  An entry's walk goes left from its end to the window start (or max_back bytes), with
+    // EndMark first (with_end, entries at the window's end only) and BeginMark last (with_begin, at the window start only).
+    const unsigned long long* entries_first;   // or null: 0
+    const unsigned long long* entries_found;
+    const uint32_t* entry_strings;   // or null: every entry belongs to string 0
+    const uint64_t* entry_ends;
+    const uint32_t* entry_ids;       // or null: Final() instead of one regexp
+    const uint64_t* window_end;
+    uint32_t with_end;               // EndMark for entries at their window's end
+    uint64_t max_back;               // 0 = no bound
+    const uint32_t* live;            // ScanTables::live, live_words per state
+    uint32_t live_words;
+    uint64_t* match_starts;          // per entry: the leftmost start, or ~0
+    uint8_t* match_open;             // per entry, or null: the walk reached its lower bound still live
+    unsigned long long* group_counter;   // scratch word, zeroed: groups of 32 entries handed out so far
 };
 
 struct LaunchPlan {
@@ -149,6 +166,9 @@ cudaError_t LaunchCount(const ScanArgs& a, int device, cudaStream_t stream, bool
 // `from`, string i's entries from index *a.found + (the entries of strings 0..i-1) on, placed by a scan over the strings;
 // then match bits, states and a.pos as LaunchCount's, and *a.found advanced by the call's total
 cudaError_t LaunchMatchEndsBatch(const ScanArgs& a, int device, cudaStream_t stream);
+// The leftmost start of every match-ends entry (MatchStartsKernel): one entry per lane, walked leftwards through a
+// reversed scanner from its end, groups of 32 entries handed to warps of a persistent grid
+cudaError_t LaunchMatchStarts(const ScanArgs& a, int device, cudaStream_t stream);
 // d_order <- string indices, longest half-octave length bucket first, corpus order inside a bucket (stable CUB radix sort).
 // stream-ordered scratch from the library's own per-device pool (see scan_kernels.cu)
 cudaError_t ScratchAlloc(void** out, size_t bytes, cudaStream_t stream);

@@ -850,6 +850,75 @@ class BatchMatchEnds:
         return self.StateTensor().cpu().numpy().view(np.uint32)
 
 
+NO_START = 0xFFFFFFFFFFFFFFFF
+
+
+class MatchStartsResult:
+    """What ``MatchStarts`` wrote: per match-ends entry, the leftmost start of its match and whether that start could
+    move further left with more bytes on the left of the window.  ``StartsTensor()`` and ``OpenTensor()`` do not
+    synchronise; ``Starts()`` and ``Open()`` do."""
+
+    def __init__(self, ends, starts, open_):
+        self._ends, self._starts, self._open = ends, starts, open_
+
+    def StartsTensor(self):
+        """The device tensor of starts (int64 holding u64, NO_START = none), the ends' ``capacity`` long; entries whose
+        end lies outside the window keep NO_START."""
+        return self._starts
+
+    def OpenTensor(self):
+        """The device tensor (uint8) of open flags, the ends' ``capacity`` long."""
+        return self._open
+
+    def Starts(self):
+        """The first min(Found(), capacity) starts, as numpy u64."""
+        k = min(self._ends.Found(), self._ends.capacity)
+        return self._starts[:k].cpu().numpy().view(np.uint64)
+
+    def Open(self):
+        """The first min(Found(), capacity) open flags, as numpy bool."""
+        k = min(self._ends.Found(), self._ends.capacity)
+        return self._open[:k].cpu().numpy().astype(bool)
+
+
+def MatchStarts(rsc, ends, window, base=0, begin=True, end=True, max_back=0):
+    """Where the matches ``ends`` lists start (pire_gpu_match_starts_string / _batch): Pire::LongestSuffix through
+    ``rsc``, a Scanner of the same patterns built with Fsm::Reverse() (glued in the same order), walked leftwards from
+    each entry's end and testing the entry's regexp id.  ``ends`` is a ``StringMatchEnds`` whose window is a uint8 CUDA
+    tensor holding the text bytes at positions [base, base + numel), or a ``BatchMatchEnds`` whose window is the
+    ``Batch`` of its last round (each stream's window ends where ``PosTensor()`` says).  ``begin`` says that the window
+    starts where the text begins (BeginMark), ``end`` that the text ended with End() (EndMark); ``max_back`` > 0 bounds
+    every walk.  Entries outside the window are left as NO_START.  Launches on the current stream, no synchronise."""
+    torch = _torch()
+    flags = (N.RUN_BEGIN if begin else 0) | (N.RUN_END if end else 0)
+    if not isinstance(ends, (StringMatchEnds, BatchMatchEnds)):
+        raise TypeError("ends must be a StringMatchEnds or a BatchMatchEnds")
+    dev = ends.EndsTensor().device
+    starts = torch.full((ends.capacity,), -1, dtype=torch.int64, device=dev)
+    open_ = torch.zeros(ends.capacity, dtype=torch.uint8, device=dev)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    if ends.capacity == 0:
+        pass                                              # no entries to walk (and no buffers to pass)
+    elif isinstance(ends, StringMatchEnds):
+        if window.dtype != torch.uint8 or not window.is_cuda or not window.is_contiguous() or window.device != dev:
+            raise ValueError("window must be a contiguous uint8 CUDA tensor on the scanner's device")
+        N.check(N.lib.pire_gpu_match_starts_string(rsc._h, window.data_ptr(), window.numel(), int(base), flags, int(max_back),
+                                                   ends.EndsTensor().data_ptr(), ends.IdsTensor().data_ptr(), None,
+                                                   ends.FoundTensor().data_ptr(), ends.capacity, starts.data_ptr(),
+                                                   open_.data_ptr(), stream), "pire_gpu_match_starts_string")
+    else:
+        if window.trim or window.order is not None or window.n != ends.n or window.device != dev:
+            raise ValueError("window must be a plain batch of the ends' n streams on the scanner's device")
+        N.check(N.lib.pire_gpu_match_starts_batch(rsc._h, window.corpus.data_ptr(),
+                                                  None if window.offsets is None else window.offsets.data_ptr(),
+                                                  window.fixed_len, window.n, ends.PosTensor().data_ptr(), flags,
+                                                  int(max_back), ends.StringsTensor().data_ptr(), ends.EndsTensor().data_ptr(),
+                                                  ends.IdsTensor().data_ptr(), None, ends.FoundTensor().data_ptr(),
+                                                  ends.capacity, starts.data_ptr(), open_.data_ptr(), stream),
+                "pire_gpu_match_starts_batch")
+    return MatchStartsResult(ends, starts, open_)
+
+
 def Runner(sc, states=None):
     """Pire::Runner(sc) (run.h:388-389); with ``states`` Pire::Runner(sc, st) (run.h:391-392) for every string."""
     return RunHelper(sc, states)
