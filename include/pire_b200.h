@@ -194,6 +194,34 @@ int pire_gpu_run_batch_from(const pire_gpu_scanner* sc,
                             uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx,
                             void* stream);
 
+/* Two scanners over one batch.  Replaces, for every string i of a batch,
+ *     Pire::Run(sc1, sc2, st1_i, st2_i, begin, end)                                        run.h:230-241
+ *     Pire::Runner(Pire::ScannerPair(sc1, sc2)) [.Begin()] .Run(string i) [.End()]         scanners/pair.h
+ * for a pattern set split over two scanners (Scanner::Glue stops at a size limit).  Each scanner's half of the result
+ * is exactly what it gets alone on the same bytes: pire_gpu_run_batch_from(sc1, ..., d_start1, outputs 1) and the same
+ * for sc2, or pire_gpu_run_batch when that scanner's start array is NULL.  ScannerPair's Final() is the OR of the two
+ * match bits.
+ *   Batch   as pire_gpu_run_batch: CSR (d_offsets) or fixed length; no order.
+ *   flags   PIRE_GPU_RUN_BEGIN and/or PIRE_GPU_RUN_END, stepped for both scanners; anything else (PIRE_GPU_RUN_LINES
+ *           included) is PIRE_GPU_EINVAL, as are a NULL corpus with non-empty strings and n > 2^40.
+ *   Start   d_start1 / d_start2: n device words each, or NULL for Initialize().  A start >= Size() yields match 0, mask
+ *           0 and state 0xFFFFFFFF for its own scanner only.
+ *   Chain   d_state_idx1 may be d_start1 and d_state_idx2 may be d_start2: both halves of a batch of streams are updated
+ *           in place round after round.  A buffer shared between the two scanners (d_state_idx2 == d_start1, say) is
+ *           not supported.
+ *   Output  as pire_gpu_run_batch, once per scanner; each of the six may be NULL.
+ *   Handles both on one device (PIRE_GPU_EINVAL otherwise); a host-only handle gets PIRE_GPU_ENODEVICE.  sc1 may be
+ *           sc2.  Each handle runs with its own hot set, tuned or not.
+ * A uniform batch (fixed length a multiple of 32, corpus 32-byte aligned) is scanned in one pass: every byte is read
+ * from HBM once and walked through both automata.  Any other batch is not fused: it runs as the two single-scanner
+ * launches, one after the other on the stream.  n == 0 is a no-op.  Asynchronous on `stream`; re-entrant. */
+int pire_gpu_run_pair_batch(const pire_gpu_scanner* sc1, const pire_gpu_scanner* sc2,
+                            const uint8_t* d_corpus, const uint64_t* d_offsets, uint64_t fixed_len, uint64_t n,
+                            uint32_t flags, const uint32_t* d_start1, const uint32_t* d_start2,
+                            uint32_t* d_match_bits1, uint32_t* d_accept_masks1, uint32_t* d_state_idx1,
+                            uint32_t* d_match_bits2, uint32_t* d_accept_masks2, uint32_t* d_state_idx2,
+                            void* stream);
+
 /* Replaces, per string of a batch,
  *     Pire::LongestPrefix(sc, begin, end, throughBeginMark, throughEndMark)   run.h:277-292
  *     Pire::ShortestPrefix(sc, begin, end, throughBeginMark, throughEndMark)   run.h:294-311

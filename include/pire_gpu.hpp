@@ -224,6 +224,80 @@ inline BatchRunner Runner(const Scanner& sc) { return BatchRunner(sc); }     // 
 // run.h:391-392, for every string of a batch
 inline BatchRunner Runner(const Scanner& sc, BatchRunner::StartWords start) { return BatchRunner(sc, start); }
 
+// Pire::ScannerPair<S1, S2> (scanners/pair.h): two scanners stepped over the same bytes.  Both on one device; they may
+// be the same Scanner.  Neither is owned.
+class ScannerPair {
+public:
+    ScannerPair(const Scanner& first, const Scanner& second) : Sc1(&first), Sc2(&second) {}
+    const Scanner& First() const { return *Sc1; }
+    const Scanner& Second() const { return *Sc2; }
+
+private:
+    const Scanner* Sc1;
+    const Scanner* Sc2;
+};
+
+// One scanner's device outputs of a pair run, each may be null (pire_gpu_run_batch's three).
+struct RunOutputs {
+    uint32_t* MatchBits = nullptr;
+    uint32_t* AcceptMasks = nullptr;
+    uint32_t* StateIdx = nullptr;
+};
+
+// Pire::RunHelper<ScannerPair> (run.h:365-386) for a device batch: one launch scans the batch for both scanners
+// (pire_gpu_run_pair_batch); Final() of the pair is the OR of the two match bits.
+//     Runner(pair).Begin().Run(batch).End().Launch(out1, out2, stream);
+//     Runner(pair, BatchRunner::From(d_st1), BatchRunner::From(d_st2)).Run(piece).Launch({nullptr, nullptr, d_st1},
+//                                                                                         {nullptr, nullptr, d_st2});
+// A null From() starts that scanner's strings from Initialize().  Each scanner's states may chain in place; a buffer
+// shared between the two scanners is not supported.
+class PairRunner {
+public:
+    explicit PairRunner(const ScannerPair& pair) : Pair(pair), Start1(nullptr), Start2(nullptr), Flags(0), Ran(false) {}
+    PairRunner(const ScannerPair& pair, BatchRunner::StartWords start1, BatchRunner::StartWords start2) : PairRunner(pair)
+    {
+        Start1 = start1.Words;
+        Start2 = start2.Words;
+    }
+
+    PairRunner& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }       // run.h:375
+    PairRunner& End() { Flags |= PIRE_GPU_RUN_END; return *this; }           // run.h:376
+    PairRunner& Run(const Batch& b) { Input = b; Ran = true; return *this; }  // run.h:372
+
+    void Launch(const RunOutputs& out1, const RunOutputs& out2, void* stream = nullptr) const
+    {
+        if (!Ran)
+            throw Error(PIRE_GPU_EINVAL, "PairRunner::Run() was not called");
+        Check(pire_gpu_run_pair_batch(Pair.First().Raw(), Pair.Second().Raw(), Input.Corpus, Input.Offsets, Input.FixedLen,
+                                      Input.Count, Flags, Start1, Start2, out1.MatchBits, out1.AcceptMasks, out1.StateIdx,
+                                      out2.MatchBits, out2.AcceptMasks, out2.StateIdx, stream),
+              "pire_gpu_run_pair_batch");
+    }
+
+private:
+    ScannerPair Pair;
+    const uint32_t* Start1;
+    const uint32_t* Start2;
+    Batch Input;
+    unsigned Flags;
+    bool Ran;
+};
+
+inline PairRunner Runner(const ScannerPair& pair) { return PairRunner(pair); }
+inline PairRunner Runner(const ScannerPair& pair, BatchRunner::StartWords start1, BatchRunner::StartWords start2)
+{
+    return PairRunner(pair, start1, start2);
+}
+
+// Pire::Run(sc1, sc2, st1, st2, begin, end) (run.h:230-241) for every string of a batch: no marks, the states in
+// d_state1 / d_state2 (n words each, StateIndex) read and updated in place.
+inline void Run(const Scanner& sc1, const Scanner& sc2, uint32_t* d_state1, uint32_t* d_state2, const Batch& b, void* stream = nullptr)
+{
+    Check(pire_gpu_run_pair_batch(sc1.Raw(), sc2.Raw(), b.Corpus, b.Offsets, b.FixedLen, b.Count, 0, d_state1, d_state2, nullptr,
+                                  nullptr, d_state1, nullptr, nullptr, d_state2, stream),
+          "pire_gpu_run_pair_batch");
+}
+
 // Counterpart of Pire::RunHelper (run.h:365-392) for ONE string resident in HBM, scanned by the whole GPU
 // (pire_gpu_run_string).  Run() may be called many times: the pieces are scanned as one string, the state carried in
 // the caller-owned device word d_state (StateIndex, reference numbering), so chained calls do not synchronise.  Every

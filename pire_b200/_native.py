@@ -39,7 +39,7 @@ SYMBOLS = [
     "pire_gpu_comm_adopt", "pire_gpu_comm_destroy", "pire_gpu_comm_info", "pire_gpu_comm_wait", "pire_gpu_run_sharded", "pire_gpu_comm_gather_bits",
     "pire_gpu_run_string", "pire_gpu_run_batch_from", "pire_gpu_count_string", "pire_gpu_count_batch_from",
     "pire_gpu_match_ends_string", "pire_gpu_match_ends_batch_from",
-    "pire_gpu_match_starts_string", "pire_gpu_match_starts_batch",
+    "pire_gpu_match_starts_string", "pire_gpu_match_starts_batch", "pire_gpu_run_pair_batch",
 ]
 
 
@@ -72,6 +72,7 @@ def _load():
     lib.pire_gpu_run_batch.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp]
     lib.pire_gpu_run_string.argtypes = [vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp]
     lib.pire_gpu_run_batch_from.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp]
+    lib.pire_gpu_run_pair_batch.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.pire_gpu_run_batch_host.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp]
     lib.pire_gpu_prefix_batch.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp]
     lib.pire_gpu_suffix_batch.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp]

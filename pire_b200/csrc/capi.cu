@@ -601,6 +601,52 @@ int pire_gpu_run_batch_from(const pire_gpu_scanner* sc, const uint8_t* d_corpus,
     return RunBatch(sc, d_corpus, d_offsets, fixed_len, n, flags, d_start, d_match_bits, d_accept_masks, d_state_idx, stream);
 }
 
+int pire_gpu_run_pair_batch(const pire_gpu_scanner* sc1, const pire_gpu_scanner* sc2, const uint8_t* d_corpus,
+                            const uint64_t* d_offsets, uint64_t fixed_len, uint64_t n, uint32_t flags, const uint32_t* d_start1,
+                            const uint32_t* d_start2, uint32_t* d_match_bits1, uint32_t* d_accept_masks1, uint32_t* d_state_idx1,
+                            uint32_t* d_match_bits2, uint32_t* d_accept_masks2, uint32_t* d_state_idx2, void* stream)
+{
+    int rc = CheckRunnable(sc1);
+    if (rc == PIRE_GPU_OK)
+        rc = CheckRunnable(sc2);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (sc1->device != sc2->device)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_run_pair_batch needs two handles on one device");
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_run_pair_batch takes PIRE_GPU_RUN_BEGIN and PIRE_GPU_RUN_END only");
+    if (n == 0)
+        return PIRE_GPU_OK;
+    if (!d_corpus && (d_offsets || fixed_len != 0))
+        return Fail(PIRE_GPU_EINVAL, "null corpus with non-empty strings");
+    if (n > (1ull << 40))
+        return Fail(PIRE_GPU_EINVAL, "too many strings");
+    if (!IsUniform(d_corpus, d_offsets, fixed_len)) {
+        // not fused: each scanner's own batch launch, one after the other on the stream
+        rc = RunBatch(sc1, d_corpus, d_offsets, fixed_len, n, flags, d_start1, d_match_bits1, d_accept_masks1, d_state_idx1, stream);
+        if (rc != PIRE_GPU_OK)
+            return rc;
+        return RunBatch(sc2, d_corpus, d_offsets, fixed_len, n, flags, d_start2, d_match_bits2, d_accept_masks2, d_state_idx2, stream);
+    }
+    CUDA_TRY(cudaSetDevice(sc1->device));
+    ScanArgs a[2];
+    const pire_gpu_scanner* sc[2] = {sc1, sc2};
+    const uint32_t* start[2] = {d_start1, d_start2};
+    uint32_t* bits[2] = {d_match_bits1, d_match_bits2};
+    uint32_t* masks[2] = {d_accept_masks1, d_accept_masks2};
+    uint32_t* states[2] = {d_state_idx1, d_state_idx2};
+    for (int k = 0; k < 2; ++k) {
+        FillArgs(sc[k], &a[k], d_corpus, nullptr, fixed_len, n, flags);
+        a[k].match_bits = bits[k];
+        a[k].accept_masks = masks[k];
+        a[k].state_idx = states[k];
+        if (start[k])
+            SetStarts(sc[k], &a[k], start[k], flags);
+    }
+    CUDA_TRY(LaunchPair(a[0], a[1], sc1->device, static_cast<cudaStream_t>(stream)));
+    return PIRE_GPU_OK;
+}
+
 int pire_gpu_run_batch_ordered(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,
                                const uint32_t* d_order, uint64_t n, uint32_t flags,
                                uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx, void* stream)

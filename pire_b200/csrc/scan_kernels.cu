@@ -629,10 +629,12 @@ __device__ __forceinline__ uint32_t SmemWindowBase()
 // Lane state in two registers: g (hot id, H = outside the hot rows) and prev = the complete state the lane had when
 // the block began (its cold state while g == H, else g itself) -- exactly what a replay starts from.
 // The replay of a whole 32-byte block for the LOOK kernels: out of line, and with every table pointer read from the
-// kernel's parameter block in here, so that the walk loop around the (rare) call carries no argument set-up.
+// kernel's parameter block in here, so that the walk loop around the (rare) call carries no argument set-up.  kAt: where
+// the tables sit in the shared array (ScanPairKernel keeps its second scanner's kPairSecond bytes in).
+template <uint32_t kAt = 0>
 __device__ __noinline__ uint32_t ReplayBlock32(const ScanArgs* a, uint32_t from, uint4 v0, uint4 v1)
 {
-    const SharedView sv = CarveShared(pire_b200_smem, a->hot);
+    const SharedView sv = CarveShared(pire_b200_smem + kAt, a->hot);
     const uint32_t letters_wide = a->letters | (a->wide << 31);
     const uint32_t mid = ReplayChunk(sv.hot, sv.cls, a->full, a->hot, letters_wide, from, v0);
     return ReplayChunk(sv.hot, sv.cls, a->full, a->hot, letters_wide, mid, v1);
@@ -766,74 +768,90 @@ __global__ void __maxnreg__(kRegs) ScanUniformLookKernel(const __grid_constant__
 // run it faster -- it is short of independent chains, and registers (48 per thread) cap the warps.  Here every lane walks TWO strings (units 2p and 2p+1 of the
 // batch) step by step in turn: the second string's step fills the latency of the first one's table read, and the
 // block bookkeeping is shared.
+// Chain a walks with (basea, fa), chain b with (baseb, fb): one table for two strings (LookBlock32x2's first form), or
+// two tables for one string (ScanPairKernel).
 template <bool kClean>
-__device__ __forceinline__ void LookWord2(uint32_t& ga, uint32_t wa, uint32_t bba0, uint32_t paa0, uint32_t pana, uint32_t& gb, uint32_t wb,
-                                          uint32_t bbb0, uint32_t pab0, uint32_t panb, uint32_t base, const LookFilter& f)
+__device__ __forceinline__ void LookWord2(uint32_t& ga, uint32_t wa, uint32_t bba0, uint32_t paa0, uint32_t pana, uint32_t basea,
+                                          const LookFilter& fa, uint32_t& gb, uint32_t wb, uint32_t bbb0, uint32_t pab0, uint32_t panb,
+                                          uint32_t baseb, const LookFilter& fb)
 {
     uint32_t bba1, bba2, bba3, paa1, paa2, paa3, bbb1, bbb2, bbb3, pab1, pab2, pab3;
-    LookProbe<false, 1, kClean>(wa, base, f, bba1, paa1);
-    LookProbe<false, 1, kClean>(wb, base, f, bbb1, pab1);
+    LookProbe<false, 1, kClean>(wa, basea, fa, bba1, paa1);
+    LookProbe<false, 1, kClean>(wb, baseb, fb, bbb1, pab1);
     LookStep<kClean>(ga, bba0, paa0, paa1);
     LookStep<kClean>(gb, bbb0, pab0, pab1);
-    LookProbe<false, 2, kClean>(wa, base, f, bba2, paa2);
-    LookProbe<false, 2, kClean>(wb, base, f, bbb2, pab2);
+    LookProbe<false, 2, kClean>(wa, basea, fa, bba2, paa2);
+    LookProbe<false, 2, kClean>(wb, baseb, fb, bbb2, pab2);
     LookStep<kClean>(ga, bba1, paa1, paa2);
     LookStep<kClean>(gb, bbb1, pab1, pab2);
-    LookProbe<false, 3, kClean>(wa, base, f, bba3, paa3);
-    LookProbe<false, 3, kClean>(wb, base, f, bbb3, pab3);
+    LookProbe<false, 3, kClean>(wa, basea, fa, bba3, paa3);
+    LookProbe<false, 3, kClean>(wb, baseb, fb, bbb3, pab3);
     LookStep<kClean>(ga, bba2, paa2, paa3);
     LookStep<kClean>(gb, bbb2, pab2, pab3);
     LookStep<kClean>(ga, bba3, paa3, pana);
     LookStep<kClean>(gb, bbb3, pab3, panb);
 }
 
+// One table and one filter per chain: chain a reads (ta, fa) and is replayed from argsa's tables, chain b reads (tb, fb)
+// and is replayed from argsb's, kAtB bytes into the shared array (ReplayBlock32).
 // `late(ga, gb, latea, lateb)` fetches the first words of the blocks that follow, after the walk of the block's first 28
-// bytes (see LookBlock32), from the ring in shared memory (ScanUniformLookRingKernel).
+// bytes (see LookBlock32), from the ring in shared memory (ScanUniformLookRingKernel, ScanPairKernel).
+template <bool kClean, uint32_t kAtB, typename Late>
+__device__ __forceinline__ void LookBlock32x2(const Tables& ta, const LookFilter& fa, const ScanArgs* argsa, uint32_t& ga, uint32_t& preva,
+                                              const uint4& a0, const uint4& a1, const Tables& tb, const LookFilter& fb,
+                                              const ScanArgs* argsb, uint32_t& gb, uint32_t& prevb, const uint4& b0, const uint4& b1,
+                                              bool more, Late late)
+{
+    preva = ga == ta.H ? preva : ga;
+    prevb = gb == tb.H ? prevb : gb;
+    uint32_t bba, paa, bna, pna, bbb, pab, bnb, pnb;
+    LookProbe<false, 0, kClean>(a0.x, ta.base, fa, bba, paa);
+    LookProbe<false, 0, kClean>(b0.x, tb.base, fb, bbb, pab);
+    LookProbe<false, 0, kClean>(a0.y, ta.base, fa, bna, pna);
+    LookProbe<false, 0, kClean>(b0.y, tb.base, fb, bnb, pnb);
+    LookWord2<kClean>(ga, a0.x, bba, paa, pna, ta.base, fa, gb, b0.x, bbb, pab, pnb, tb.base, fb);
+    LookProbe<false, 0, kClean>(a0.z, ta.base, fa, bba, paa);
+    LookProbe<false, 0, kClean>(b0.z, tb.base, fb, bbb, pab);
+    LookWord2<kClean>(ga, a0.y, bna, pna, paa, ta.base, fa, gb, b0.y, bnb, pnb, pab, tb.base, fb);
+    LookProbe<false, 0, kClean>(a0.w, ta.base, fa, bna, pna);
+    LookProbe<false, 0, kClean>(b0.w, tb.base, fb, bnb, pnb);
+    LookWord2<kClean>(ga, a0.z, bba, paa, pna, ta.base, fa, gb, b0.z, bbb, pab, pnb, tb.base, fb);
+    LookProbe<false, 0, kClean>(a1.x, ta.base, fa, bba, paa);
+    LookProbe<false, 0, kClean>(b1.x, tb.base, fb, bbb, pab);
+    LookWord2<kClean>(ga, a0.w, bna, pna, paa, ta.base, fa, gb, b0.w, bnb, pnb, pab, tb.base, fb);
+    LookProbe<false, 0, kClean>(a1.y, ta.base, fa, bna, pna);
+    LookProbe<false, 0, kClean>(b1.y, tb.base, fb, bnb, pnb);
+    LookWord2<kClean>(ga, a1.x, bba, paa, pna, ta.base, fa, gb, b1.x, bbb, pab, pnb, tb.base, fb);
+    LookProbe<false, 0, kClean>(a1.z, ta.base, fa, bba, paa);
+    LookProbe<false, 0, kClean>(b1.z, tb.base, fb, bbb, pab);
+    LookWord2<kClean>(ga, a1.y, bna, pna, paa, ta.base, fa, gb, b1.y, bnb, pnb, pab, tb.base, fb);
+    LookProbe<false, 0, kClean>(a1.w, ta.base, fa, bna, pna);
+    LookProbe<false, 0, kClean>(b1.w, tb.base, fb, bnb, pnb);
+    LookWord2<kClean>(ga, a1.z, bba, paa, pna, ta.base, fa, gb, b1.z, bbb, pab, pnb, tb.base, fb);
+    // the words after the blocks are still on their way from HBM: their probes stay behind the walk (see LookBlock32)
+    uint32_t latea, lateb;
+    late(ga, gb, latea, lateb);
+    LookProbe<false, 0, kClean>(latea, ta.base, fa, bba, paa);
+    LookProbe<false, 0, kClean>(lateb, tb.base, fb, bbb, pab);
+    LookWord2<kClean>(ga, a1.w, bna, pna, more ? paa : 0x80000000u, ta.base, fa, gb, b1.w, bnb, pnb, more ? pab : 0x80000000u, tb.base,
+                      fb);
+    if (ga == ta.H) {
+        preva = ReplayBlock32(argsa, preva, a0, a1);
+        ga = preva < ta.H ? preva : ta.H;
+    }
+    if (gb == tb.H) {
+        prevb = ReplayBlock32<kAtB>(argsb, prevb, b0, b1);
+        gb = prevb < tb.H ? prevb : tb.H;
+    }
+}
+
+// Two strings through one table (ScanUniformLookRingKernel).
 template <bool kClean, typename Late>
 __device__ __forceinline__ void LookBlock32x2(const Tables& t, uint32_t& ga, uint32_t& preva, const uint4& a0, const uint4& a1,
                                               uint32_t& gb, uint32_t& prevb, const uint4& b0, const uint4& b1, bool more,
                                               const LookFilter& f, Late late, const ScanArgs* args)
 {
-    preva = ga == t.H ? preva : ga;
-    prevb = gb == t.H ? prevb : gb;
-    uint32_t bba, paa, bna, pna, bbb, pab, bnb, pnb;
-    LookProbe<false, 0, kClean>(a0.x, t.base, f, bba, paa);
-    LookProbe<false, 0, kClean>(b0.x, t.base, f, bbb, pab);
-    LookProbe<false, 0, kClean>(a0.y, t.base, f, bna, pna);
-    LookProbe<false, 0, kClean>(b0.y, t.base, f, bnb, pnb);
-    LookWord2<kClean>(ga, a0.x, bba, paa, pna, gb, b0.x, bbb, pab, pnb, t.base, f);
-    LookProbe<false, 0, kClean>(a0.z, t.base, f, bba, paa);
-    LookProbe<false, 0, kClean>(b0.z, t.base, f, bbb, pab);
-    LookWord2<kClean>(ga, a0.y, bna, pna, paa, gb, b0.y, bnb, pnb, pab, t.base, f);
-    LookProbe<false, 0, kClean>(a0.w, t.base, f, bna, pna);
-    LookProbe<false, 0, kClean>(b0.w, t.base, f, bnb, pnb);
-    LookWord2<kClean>(ga, a0.z, bba, paa, pna, gb, b0.z, bbb, pab, pnb, t.base, f);
-    LookProbe<false, 0, kClean>(a1.x, t.base, f, bba, paa);
-    LookProbe<false, 0, kClean>(b1.x, t.base, f, bbb, pab);
-    LookWord2<kClean>(ga, a0.w, bna, pna, paa, gb, b0.w, bnb, pnb, pab, t.base, f);
-    LookProbe<false, 0, kClean>(a1.y, t.base, f, bna, pna);
-    LookProbe<false, 0, kClean>(b1.y, t.base, f, bnb, pnb);
-    LookWord2<kClean>(ga, a1.x, bba, paa, pna, gb, b1.x, bbb, pab, pnb, t.base, f);
-    LookProbe<false, 0, kClean>(a1.z, t.base, f, bba, paa);
-    LookProbe<false, 0, kClean>(b1.z, t.base, f, bbb, pab);
-    LookWord2<kClean>(ga, a1.y, bna, pna, paa, gb, b1.y, bnb, pnb, pab, t.base, f);
-    LookProbe<false, 0, kClean>(a1.w, t.base, f, bna, pna);
-    LookProbe<false, 0, kClean>(b1.w, t.base, f, bnb, pnb);
-    LookWord2<kClean>(ga, a1.z, bba, paa, pna, gb, b1.z, bbb, pab, pnb, t.base, f);
-    // the words after the blocks are still on their way from HBM: their probes stay behind the walk (see LookBlock32)
-    uint32_t latea, lateb;
-    late(ga, gb, latea, lateb);
-    LookProbe<false, 0, kClean>(latea, t.base, f, bba, paa);
-    LookProbe<false, 0, kClean>(lateb, t.base, f, bbb, pab);
-    LookWord2<kClean>(ga, a1.w, bna, pna, more ? paa : 0x80000000u, gb, b1.w, bnb, pnb, more ? pab : 0x80000000u, t.base, f);
-    if (ga == t.H) {
-        preva = ReplayBlock32(args, preva, a0, a1);
-        ga = preva < t.H ? preva : t.H;
-    }
-    if (gb == t.H) {
-        prevb = ReplayBlock32(args, prevb, b0, b1);
-        gb = prevb < t.H ? prevb : t.H;
-    }
+    LookBlock32x2<kClean, 0>(t, f, args, ga, preva, a0, a1, t, f, args, gb, prevb, b0, b1, more, late);
 }
 
 // ---------------------------------------------------------------- LOOK variant, two strings per lane, fed from a ring
@@ -1115,6 +1133,134 @@ __global__ void __launch_bounds__(kRing1Block, 1) ScanUniformLookRing1Kernel(con
         s.g = t.H;
         s.cold = g == t.H ? prev : g;
         Report(a, t, s, unit, i, i < a.n, known);
+    }
+}
+
+// ---------------------------------------------------------------- two scanners over one batch, fed from a ring
+//
+// Pire::Run(sc1, sc2, ...) / Runner(ScannerPair) (run.h:230-241, scanners/pair.h) for a uniform batch: every byte is
+// copied from HBM once and walked through both automata.  One string per lane, fed from a ring as in
+// ScanUniformLookRing1Kernel; each byte advances two look-ahead chains, one per scanner, in LookBlock32x2's order, so the
+// second scanner's step fills the latency of the first one's table read as the second string did in
+// ScanUniformLookRingKernel.  Shared memory: the first scanner's tables at 0, the second's at kPairSecond (room for any
+// hot set), then 24 warps x 3 slots of 1 KB: 225 040 bytes at most, within the 227 KB a block may have on sm_90, so
+// neither hot set is cut.  A warp leaves a unit early only when every lane sits in a NoExit state of both scanners.
+struct PairArgs {
+    ScanArgs s[2];
+};
+constexpr int kPairBlock = 768;
+constexpr int kPairSlots = 3;
+constexpr uint32_t kPairSecond = ((kMaxHot + 1 + 3) / 4 * 4 * kHotStride + 512 + 256 + 16 + 255) / 256 * 256;   // 75 776
+
+// The first word of the next block for both chains, read once after the walk of this block's first 28 bytes; the address
+// depends on chain a's walk and the word handed to chain b on chain b's (see RingNext).
+struct RingPairNext {
+    uint32_t at;          // the next block's slot
+    uint32_t zero;
+    __device__ __forceinline__ void operator()(uint32_t ga, uint32_t gb, uint32_t& latea, uint32_t& lateb) const
+    {
+        CopyAsyncWait<kPairSlots - 1>();
+        latea = LoadShared4(at + ga * zero);
+        lateb = latea + gb * zero;
+    }
+};
+
+__device__ __forceinline__ void PairTables(const ScanArgs& a, const SharedView& sv, uint32_t base, Tables& t, LookFilter& f)
+{
+    t.hot = sv.hot;
+    t.base = base;
+    t.cls = sv.cls;
+    t.full = a.full;
+    t.H = a.hot;
+    t.letters = a.letters;
+    t.wide = a.wide;
+    t.m0 = a.look_bitmap;
+    f.lo = a.look_bitmap;     // all ones for a scanner without a look-ahead set: its chain reads the table on every byte
+    f.hi = 0;
+    f.zero = a.opaque_zero;
+    f.rev = __brev(f.lo);
+}
+
+__global__ void __launch_bounds__(kPairBlock, 1) ScanPairKernel(const __grid_constant__ PairArgs p)
+{
+    const ScanArgs& a = p.s[0];
+    const ScanArgs& b = p.s[1];
+    uint8_t* const smem = pire_b200_smem;
+    const SharedView sva = CarveShared(smem, a.hot);
+    const SharedView svb = CarveShared(smem + kPairSecond, b.hot);
+    StageTables(a, sva, a.hot8, a.hot);
+    StageTables(b, svb, b.hot8, b.hot);
+
+    Tables ta, tb;
+    LookFilter fa, fb;
+    PairTables(a, sva, SmemWindowBase(), ta, fa);
+    PairTables(b, svb, SmemWindowBase() + kPairSecond, tb, fb);
+
+    const uint32_t units = (uint32_t) ((a.n + 31) / 32);
+    const uint32_t warps_per_block = blockDim.x >> 5;
+    const uint32_t warps = gridDim.x * warps_per_block;
+    const uint32_t len = (uint32_t) a.fixed_len;
+    const uint32_t blocks = len >> 5;
+    // this lane's 16-byte column of its warp's ring (slot 0, first half), behind the second scanner's tables
+    const uint32_t ring = SmemAddr(svb.stage) + (threadIdx.x >> 5) * (uint32_t) (kPairSlots * kRing1SlotBytes) + (threadIdx.x & 31) * 16;
+
+    for (uint32_t unit = blockIdx.x * warps_per_block + (threadIdx.x >> 5); unit < units; unit += warps) {
+        uint32_t ga, preva, gb, prevb;
+        bool knowna, knownb;
+        {
+            const uint64_t i = (uint64_t) unit * 32 + (threadIdx.x & 31);
+            const uint8_t* q = a.corpus + (i < a.n ? i : a.n - 1) * (uint64_t) len;
+            // a scanner without starts runs from a.start / b.start (Initialize(), BeginMark stepped with BEGIN)
+            preva = LaneStart<true>(a, ta, i, i < a.n && a.starts, knowna);
+            prevb = LaneStart<true>(b, tb, i, i < b.n && b.starts, knownb);
+            ga = preva < ta.H ? preva : ta.H;
+            gb = prevb < tb.H ? prevb : tb.H;
+            if (blocks != 0) {
+                // the ring of ScanUniformLookRing1Kernel: blocks 0..kPairSlots-1, then block k + kPairSlots into the slot
+                // of block k as soon as block k is in registers; no copy reaches past the end of a string
+#pragma unroll
+                for (uint32_t j = 0; j < kPairSlots; ++j) {
+                    if (j < blocks)
+                        CopyBlock32(ring + j * kRing1SlotBytes, q + 32 * j);
+                    CopyAsyncCommit();
+                }
+                CopyAsyncWait<kPairSlots - 1>();                    // block 0 has landed
+                uint32_t s0 = 0;                                    // slot of block k
+                for (uint32_t k = 0;; k += 2) {
+                    const uint32_t s1 = NextSlot1<kPairSlots>(s0);
+                    uint4 v0 = LoadShared16(ring + s0), v1 = LoadShared16(ring + s0 + 512);
+                    if (k + kPairSlots < blocks)
+                        CopyBlock32(ring + s0, q + 32 * (size_t) (k + kPairSlots));
+                    CopyAsyncCommit();
+                    const bool more_1 = k + 1 < blocks;
+                    LookBlock32x2<true, kPairSecond>(ta, fa, &a, ga, preva, v0, v1, tb, fb, &b, gb, prevb, v0, v1, more_1,
+                                                     RingPairNext{ring + s1, a.opaque_zero});
+                    if (!more_1)
+                        break;
+                    const uint32_t s2 = NextSlot1<kPairSlots>(s1);
+                    v0 = LoadShared16(ring + s1), v1 = LoadShared16(ring + s1 + 512);
+                    if (k + 1 + kPairSlots < blocks)
+                        CopyBlock32(ring + s1, q + 32 * (size_t) (k + 1 + kPairSlots));
+                    CopyAsyncCommit();
+                    const bool more_2 = k + 2 < blocks;
+                    LookBlock32x2<true, kPairSecond>(ta, fa, &a, ga, preva, v0, v1, tb, fb, &b, gb, prevb, v0, v1, more_2,
+                                                     RingPairNext{ring + s2, a.opaque_zero});
+                    // multi.h:955-958,:979-982 (NoExit) in both scanners, looked at every 64 bytes
+                    if (!more_2 || __all_sync(0xffffffffu, (sva.noexit[ga] & svb.noexit[gb]) != 0))
+                        break;
+                    s0 = s2;
+                }
+                CopyAsyncWait<0>();            // a NoExit exit leaves copies in flight: they land before the slots are reused
+            }
+        }
+        const uint64_t i = (uint64_t) unit * 32 + (threadIdx.x & 31);
+        LaneState s;
+        s.g = ta.H;
+        s.cold = ga == ta.H ? preva : ga;
+        Report(a, ta, s, unit, i, i < a.n, knowna);
+        s.g = tb.H;
+        s.cold = gb == tb.H ? prevb : gb;
+        Report(b, tb, s, unit, i, i < b.n, knownb);
     }
 }
 
@@ -4219,7 +4365,38 @@ cudaError_t PrepareScanKernels(int device)
                 if (err != cudaSuccess)
                     return err;
             }
-    return cudaSuccess;
+    err = cudaFuncSetAttribute(reinterpret_cast<const void*>(&ScanPairKernel), cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+    if (err == cudaSuccess)
+        err = cudaFuncSetAttribute(reinterpret_cast<const void*>(&ScanPairKernel), cudaFuncAttributePreferredSharedMemoryCarveout,
+                                   cudaSharedmemCarveoutMaxShared);
+    return err;
+}
+
+cudaError_t LaunchPair(const ScanArgs& a, const ScanArgs& b, int device, cudaStream_t stream)
+{
+    if (a.n == 0)
+        return cudaSuccess;
+    const void* fn = reinterpret_cast<const void*>(&ScanPairKernel);
+    const size_t shared = kPairSecond + ScanSharedBytes(b.hot, 0) + (size_t) (kPairBlock / 32) * kPairSlots * kRing1SlotBytes;
+    int sms = 0, per_sm = 0;
+    cudaError_t err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err == cudaSuccess)
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kPairBlock, shared);
+    if (err != cudaSuccess)
+        return err;
+    if (per_sm < 1)
+        return cudaErrorLaunchOutOfResources;
+    const uint64_t units = (a.n + 31) / 32;
+    const uint64_t want = (units + kPairBlock / 32 - 1) / (kPairBlock / 32);
+    const uint64_t cap = (uint64_t) sms * (uint64_t) per_sm;
+    PairArgs p;
+    p.s[0] = a;
+    p.s[1] = b;
+    void* args[] = {&p};
+    err = cudaLaunchKernel(fn, dim3((unsigned) (want < cap ? want : cap)), dim3(kPairBlock), args, shared, stream);
+    if (err == cudaSuccess)
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+    return err;
 }
 
 cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv_rows, int variant, bool uniform, LaunchPlan* plan,

@@ -139,6 +139,9 @@ cudaError_t PlanScan(int device, uint32_t hot, uint32_t hot_small, uint32_t priv
                      bool starts = false);
 // a.starts selects the kernels that start every string from its own state
 cudaError_t LaunchScan(const ScanArgs& a, int variant, bool uniform, const LaunchPlan& plan, cudaStream_t stream);
+// Two scanners over one uniform batch (ScanPairKernel, pire_gpu_run_pair_batch): a and b are what LaunchScan would take
+// for each scanner alone (the same corpus, fixed_len and n); a.starts / b.starts may each be null
+cudaError_t LaunchPair(const ScanArgs& a, const ScanArgs& b, int device, cudaStream_t stream);
 // CSR batches of short strings (lines of text): lanes pull strings dynamically; a.match_bits must be zeroed
 cudaError_t LaunchLines(const ScanArgs& a, int variant, int device, cudaStream_t stream);
 // length-ordered CSR batches: the leading long strings, one per warp; sets *a.split_count, which the generic launch honours

@@ -42,6 +42,13 @@ check(sc, orc, batch, host, None, 256, n, "glue10 tuned")
 sc.set_max_hot(3)
 check(sc, orc, batch, host, None, 256, n, "glue10 hot=3")
 print(sc.AutoSelect(batch))
+# the same batch through glue10 (hot=3) and a full glue10 handle at once (ScanPairKernel), against the oracle
+full = P.Scanner(img, 0)
+pr = P.Runner(P.ScannerPair(sc, full)).Begin().Run(batch).End()
+f, m, s = orc.run(host, None, fixed_len=256, n=n, shortcuts=True)
+for half in (pr.First(), pr.Second()):
+    assert (half.Matches().astype(np.uint8) == f).all() and (half.AcceptMasks() == m).all() and (half.States() == s).all(), "pair"
+print("ok pair n=%d" % n, flush=True)
 
 # UTF-8 scanner, ragged CSR batch: generic kernels, ordered launch, host entry point
 img = W.load_image("headline_iu")
