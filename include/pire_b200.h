@@ -404,7 +404,8 @@ int pire_gpu_count_batch_from(const pire_gpu_scanner* sc,
  * NULL d_found, a NULL corpus with non-empty strings and n >= 2^32 (string indices are u32) are PIRE_GPU_EINVAL; a
  * host-only handle gets PIRE_GPU_ENODEVICE.  Asynchronous on `stream`; re-entrant across streams on one handle (per-call
  * scratch).  It costs about pire_gpu_count_batch_from plus a walk of the strings that have entries, and the writes of the
- * entries (DESIGN.md 4).  Not covered, as in pire_gpu_count_batch_from: ordered batches (d_order) and line batches. */
+ * entries (DESIGN.md 4).  Not covered, as in pire_gpu_count_batch_from: ordered batches (d_order) and line batches
+ * (PIRE_GPU_RUN_LINES is refused; the lines of a text have pire_gpu_match_ends_lines). */
 int pire_gpu_match_ends_batch_from(const pire_gpu_scanner* sc,
                                    const uint8_t* d_corpus, const uint64_t* d_offsets, uint64_t fixed_len, uint64_t n,
                                    uint32_t flags, const uint32_t* d_start, uint64_t* d_pos,
@@ -439,7 +440,8 @@ int pire_gpu_match_ends_batch_from(const pire_gpu_scanner* sc,
  *   Open    d_open[k] (may be NULL) is 1 when a walk of entry k reached its lower bound in a state from which id_k
  *           (with d_ids == NULL: a final state) can still be accepted and no BeginMark step settled it: bytes further
  *           left could move the start left, so the caller may widen the window (or max_back) and call again.
- *   flags   PIRE_GPU_RUN_BEGIN and/or PIRE_GPU_RUN_END; anything else (LINES included) is PIRE_GPU_EINVAL.
+ *   flags   PIRE_GPU_RUN_BEGIN and/or PIRE_GPU_RUN_END; anything else (LINES included) is PIRE_GPU_EINVAL.  The
+ *           entries of pire_gpu_match_ends_lines have pire_gpu_match_starts_lines.
  * Nothing outside the processed index range is written.  A NULL d_ends, d_found or d_starts and a NULL text with a
  * non-empty window are PIRE_GPU_EINVAL; a host-only handle gets PIRE_GPU_ENODEVICE; n == 0 or capacity == 0 is a
  * no-op.  Asynchronous on `stream`; re-entrant across streams on one handle (per-call scratch).  One entry per lane,
@@ -476,6 +478,48 @@ int pire_gpu_split_lines(const uint8_t* d_text, uint64_t n_bytes, uint64_t* d_li
 int pire_gpu_run_lines(const pire_gpu_scanner* sc, const uint8_t* d_text, const uint64_t* d_line_offsets,
                        const uint32_t* d_order, uint64_t n_lines, uint32_t flags,
                        uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx, void* stream);
+
+/* Where the HalfFinalScanner matches end in every line of a text (grep -o, grep -n, grep -b): each line is its own run,
+ * Runner(sc).Begin().Run(line).End() as samples/pigrep runs it, listed as pire_gpu_match_ends_batch_from lists a batch.
+ *   Lines   d_line_offsets are the offsets pire_gpu_split_lines made for d_text, as pire_gpu_run_lines requires; line l
+ *           is d_text[off[l], off[l+1] - 1).
+ *   Run     every line from Initialize(), whose TakeAction is reported; with BEGIN, BeginMark is stepped and reported;
+ *           then the line's bytes; with END, EndMark is stepped and reported.  Each TakeAction yields one entry (l, end,
+ *           id) for each id in the accept list of the state entered, in list order.
+ *   Positions are the text's: Initialize() and BeginMark at off[l], byte k of line l at off[l] + k + 1, EndMark at
+ *           off[l+1] - 1.  So the entries index d_text directly, and pire_gpu_match_starts_lines takes them as they are.
+ *   Order   ascending line, then walk order within a line.  The placement comes from a scan, not from atomics: two calls
+ *           on the same input write identical bytes.
+ *   Output  as in pire_gpu_match_ends_batch_from: *d_found (required) is read and ADDED to; the call's k-th entry goes to
+ *           index *d_found + k of d_lines, d_ends and d_ids (each may be NULL) if that index is < capacity, and a short
+ *           buffer holds exactly the first `capacity` entries of the full answer while *d_found is still the full total.
+ *           d_match_bits / d_state_idx (each may be NULL) are what pire_gpu_run_lines gives with the same handle and
+ *           flags; bits past n_lines are 0.
+ *   flags   PIRE_GPU_RUN_BEGIN and/or PIRE_GPU_RUN_END; PIRE_GPU_RUN_LINES is implied and accepted; anything else is
+ *           PIRE_GPU_EINVAL.
+ * The entries of line l are exactly what pire_gpu_match_ends_string writes for that line alone (d_start NULL, the same
+ * flags, base off[l]); their per-id histogram is row l of pire_gpu_count_batch with PIRE_GPU_RUN_LINES.  A NULL d_found,
+ * NULL offsets, a NULL text with lines and n_lines >= 2^32 (line indices are u32) are PIRE_GPU_EINVAL; a host-only handle
+ * gets PIRE_GPU_ENODEVICE; n_lines == 0 is a no-op.  Asynchronous on `stream`; re-entrant across streams on one handle
+ * (per-call scratch).  The lines are walked where they lie, as in pire_gpu_run_lines, in two walks around a scan
+ * (DESIGN.md 4); a handle whose start state is not a hot row walks one line per lane.  Not covered: resuming lines
+ * across calls and ordered line batches.
+ *
+ * pire_gpu_match_starts_lines: pire_gpu_match_starts_batch for those entries, with each entry's window its own line
+ * [off[l], off[l+1] - 1) and its end and start positions of the text.  BEGIN steps BeginMark at each line's start; END
+ * walks an entry at its line's end with and without EndMark; max_back, d_open, d_first and the window rules (entries
+ * outside their line, or with l >= n_lines, are not written) are unchanged.  The answer for entry k is that of
+ * pire_gpu_match_starts_string with line l as its window and base off[l].  d_lines and the offsets are required
+ * (PIRE_GPU_EINVAL without them); PIRE_GPU_RUN_LINES is accepted. */
+int pire_gpu_match_ends_lines(const pire_gpu_scanner* sc, const uint8_t* d_text, const uint64_t* d_line_offsets,
+                              uint64_t n_lines, uint32_t flags,
+                              uint32_t* d_lines, uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity, uint64_t* d_found,
+                              uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream);
+int pire_gpu_match_starts_lines(const pire_gpu_scanner* rsc, const uint8_t* d_text, const uint64_t* d_line_offsets,
+                                uint64_t n_lines, uint32_t flags, uint64_t max_back,
+                                const uint32_t* d_lines, const uint64_t* d_ends, const uint32_t* d_ids,
+                                const uint64_t* d_first, const uint64_t* d_found, uint64_t capacity,
+                                uint64_t* d_starts, uint8_t* d_open, void* stream);
 
 /* Same call with HOST buffers -- what a Pire user holds: Run(const char* begin, const char* end) takes pageable
  * memory (run.h:271-275; samples/pigrep/pigrep.cpp:38-45).  The corpus is cut into chunks of whole 32-string

@@ -429,6 +429,9 @@ void MatchStarts(const Scanner& rsc, const StringMatchEnds& ends, const uint8_t*
                  const uint64_t* d_first = nullptr);
 void MatchStarts(const Scanner& rsc, const BatchMatchEnds& ends, const Batch& window, uint64_t* d_starts, uint8_t* d_open = nullptr,
                  bool begin = true, bool end = true, uint64_t max_back = 0, const uint64_t* d_first = nullptr);
+class LineMatchEnds;
+void MatchStarts(const Scanner& rsc, const LineMatchEnds& ends, uint64_t* d_starts, uint8_t* d_open = nullptr, bool begin = true,
+                 bool end = true, uint64_t max_back = 0, const uint64_t* d_first = nullptr);
 
 class StringMatchEnds {
 public:
@@ -630,12 +633,70 @@ private:
     bool Ran;
 };
 
-// Where the matches of a StringMatchEnds / BatchMatchEnds start (pire_gpu_match_starts_string / _batch): Pire::LongestSuffix
+// Where the matches end in every line of a text (pire_gpu_match_ends_lines): each line its own run, as
+// Runner(sc).Begin().Run(line).End() runs it, with the entries (line, end, regexp id) appended to the caller-owned device
+// arrays d_lines / d_ends / d_ids (each may be null) of `capacity` entries in line order, and their number ADDED to the
+// caller-owned device word *d_found.  Ends are positions in the text: byte k of line l ends at offsets[l] + k + 1.  The
+// batch is the text's lines (pire_gpu_split_lines's offsets, Count = the number of lines).  Run() takes the lines and
+// End() makes the one launch with EndMark on every line; Launch() makes it without.  d_state / d_match_bits (optional,
+// one word per line / per 32 lines) get what pire_gpu_run_lines gives.  No synchronise.
+//     LineMatchEnds m(gsc, d_lines, d_ends, d_ids, capacity, d_found);
+//     m.Begin().Run(lines).End();
+class LineMatchEnds {
+public:
+    LineMatchEnds(const Scanner& sc, uint32_t* d_lines, uint64_t* d_ends, uint32_t* d_ids, uint64_t capacity, uint64_t* d_found,
+                  uint32_t* d_state = nullptr, uint32_t* d_match_bits = nullptr, void* stream = nullptr)
+        : Sc(&sc), Lines(d_lines), Ends(d_ends), Ids(d_ids), Capacity(capacity), Found(d_found), State(d_state), Bits(d_match_bits),
+          Stream(stream), Text{nullptr, nullptr, 0, 0}, Flags(0), Ran(false)
+    {
+        if (!d_found)
+            throw Error(PIRE_GPU_EINVAL, "LineMatchEnds needs a device word for the number of entries");
+    }
+
+    LineMatchEnds& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }
+    LineMatchEnds& Run(const Batch& lines)
+    {
+        if (!lines.Offsets || Ran)
+            throw Error(PIRE_GPU_EINVAL, "LineMatchEnds::Run takes the lines of one text");
+        Text = lines;
+        return *this;
+    }
+    LineMatchEnds& End() { Flags |= PIRE_GPU_RUN_END; return Launch(); }
+    LineMatchEnds& Launch()
+    {
+        if (Ran)
+            throw Error(PIRE_GPU_EINVAL, "LineMatchEnds launches once");
+        Check(pire_gpu_match_ends_lines(Sc->Raw(), Text.Corpus, Text.Offsets, Text.Count, Flags, Lines, Ends, Ids, Capacity, Found,
+                                        Bits, State, Stream),
+              "pire_gpu_match_ends_lines");
+        Ran = true;
+        return *this;
+    }
+
+private:
+    friend void MatchStarts(const Scanner&, const LineMatchEnds&, uint64_t*, uint8_t*, bool, bool, uint64_t, const uint64_t*);
+
+    const Scanner* Sc;
+    uint32_t* Lines;
+    uint64_t* Ends;
+    uint32_t* Ids;
+    uint64_t Capacity;
+    uint64_t* Found;
+    uint32_t* State;
+    uint32_t* Bits;
+    void* Stream;
+    Batch Text;
+    unsigned Flags;
+    bool Ran;
+};
+
+// Where the matches of a StringMatchEnds / BatchMatchEnds / LineMatchEnds start (pire_gpu_match_starts_string / _batch): Pire::LongestSuffix
 // through `rsc`, the same patterns built with Fsm::Reverse() and glued in the same order, walked leftwards from each
 // entry's end.  d_starts (and d_open, if given) get one word per entry of the ends' buffers, for entries
 // [*d_first, min(*d_found, capacity)); entries whose end lies outside the window are not written.  String form: the
 // window holds the text bytes at positions [base, base + n_bytes).  Batch form: the window is the batch of the ends'
-// last round (string i ends where the ends' d_pos says).  begin: the window starts where the text begins; end: the
+// last round (string i ends where the ends' d_pos says).  Line form: each entry's window is its own line of the ends'
+// text (pire_gpu_match_starts_lines); d_lines must have been given.  begin: the window starts where the text begins; end: the
 // ends' run took End().  On the ends' stream, with no synchronise.
 //     StringMatchEnds m(gsc, d_ends, d_ids, cap, d_found, d_state);
 //     m.Begin().Run(d_text, n).End();
@@ -655,6 +716,15 @@ inline void MatchStarts(const Scanner& rsc, const BatchMatchEnds& ends, const Ba
                                       (begin ? PIRE_GPU_RUN_BEGIN : 0u) | (end ? PIRE_GPU_RUN_END : 0u), max_back, ends.Strings,
                                       ends.Ends, ends.Ids, d_first, ends.Found, ends.Capacity, d_starts, d_open, ends.Stream),
           "pire_gpu_match_starts_batch");
+}
+
+inline void MatchStarts(const Scanner& rsc, const LineMatchEnds& ends, uint64_t* d_starts, uint8_t* d_open, bool begin, bool end,
+                        uint64_t max_back, const uint64_t* d_first)
+{
+    Check(pire_gpu_match_starts_lines(rsc.Raw(), ends.Text.Corpus, ends.Text.Offsets, ends.Text.Count,
+                                      (begin ? PIRE_GPU_RUN_BEGIN : 0u) | (end ? PIRE_GPU_RUN_END : 0u), max_back, ends.Lines, ends.Ends,
+                                      ends.Ids, d_first, ends.Found, ends.Capacity, d_starts, d_open, ends.Stream),
+          "pire_gpu_match_starts_lines");
 }
 
 // AcceptedRegexps for scanners with more than 32 regexps: rows of AcceptWords(sc) words, bit r of row i set iff

@@ -40,6 +40,7 @@ SYMBOLS = [
     "pire_gpu_run_string", "pire_gpu_run_batch_from", "pire_gpu_count_string", "pire_gpu_count_batch_from",
     "pire_gpu_match_ends_string", "pire_gpu_match_ends_batch_from",
     "pire_gpu_match_starts_string", "pire_gpu_match_starts_batch", "pire_gpu_run_pair_batch",
+    "pire_gpu_match_ends_lines", "pire_gpu_match_starts_lines",
 ]
 
 
@@ -87,6 +88,9 @@ def _load():
                                                  C.c_uint64, vp, vp, vp]
     lib.pire_gpu_match_starts_batch.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, vp, C.c_uint32, C.c_uint64, vp, vp, vp, vp,
                                                 vp, C.c_uint64, vp, vp, vp]
+    lib.pire_gpu_match_ends_lines.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, C.c_uint64, vp, vp, vp, vp]
+    lib.pire_gpu_match_starts_lines.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint32, C.c_uint64, vp, vp, vp, vp, vp, C.c_uint64,
+                                                vp, vp, vp]
     lib.pire_gpu_length_order.argtypes = [vp, C.c_uint64, vp, C.c_int, vp]
     lib.pire_gpu_run_batch_ordered.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, vp]
     lib.pire_gpu_split_lines.argtypes = [vp, C.c_uint64, vp, C.c_uint64, C.POINTER(C.c_uint64), C.c_int, vp]

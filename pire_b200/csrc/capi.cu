@@ -546,6 +546,43 @@ int pire_gpu_match_ends_batch_from(const pire_gpu_scanner* sc, const uint8_t* d_
     return PIRE_GPU_OK;
 }
 
+int pire_gpu_match_ends_lines(const pire_gpu_scanner* sc, const uint8_t* d_text, const uint64_t* d_line_offsets,
+                              uint64_t n_lines, uint32_t flags, uint32_t* d_lines, uint64_t* d_ends, uint32_t* d_ids,
+                              uint64_t capacity, uint64_t* d_found, uint32_t* d_match_bits, uint32_t* d_state_idx, void* stream)
+{
+    int rc = CheckRunnable(sc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END | PIRE_GPU_RUN_LINES))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_match_ends_lines takes PIRE_GPU_RUN_BEGIN, PIRE_GPU_RUN_END and PIRE_GPU_RUN_LINES only");
+    if (!d_found)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_match_ends_lines needs a device word for the number of entries");
+    if (!d_line_offsets)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_match_ends_lines needs the line offsets");
+    if (n_lines == 0)
+        return PIRE_GPU_OK;
+    if (!d_text)
+        return Fail(PIRE_GPU_EINVAL, "null text with lines");
+    if (n_lines >= (1ull << 32))
+        return Fail(PIRE_GPU_EINVAL, "too many lines: line indices are u32");
+    CUDA_TRY(cudaSetDevice(sc->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ScanArgs a;
+    FillArgs(sc, &a, d_text, d_line_offsets, 0, n_lines, flags | PIRE_GPU_RUN_LINES);
+    SetCounting(sc, &a, flags);
+    a.match_bits = d_match_bits;
+    a.state_idx = d_state_idx;
+    a.strings = d_lines;
+    a.ends = d_ends;
+    a.ids = d_ids;
+    a.ends_capacity = capacity;
+    a.found = reinterpret_cast<unsigned long long*>(d_found);
+    if (d_match_bits)
+        CUDA_TRY(cudaMemsetAsync(d_match_bits, 0, (size_t) ((n_lines + 31) / 32) * 4, st));
+    CUDA_TRY(LaunchMatchEndsLines(a, sc->device, st));
+    return PIRE_GPU_OK;
+}
+
 uint32_t pire_gpu_accept_words(const pire_gpu_scanner* sc) { return sc ? sc->accept_words : 0; }
 
 int pire_gpu_accept_sets(const pire_gpu_scanner* sc, const uint32_t* d_state_idx, uint64_t n, uint32_t* d_accept_sets, void* stream)
@@ -830,10 +867,12 @@ int pire_gpu_match_ends_string(const pire_gpu_scanner* sc, const uint8_t* d_text
 }
 
 // Both match-starts entry points: the string form is a batch of one string whose window ends at base + n_bytes.
+// lines: d_offsets are a text's lines (pire_gpu_match_starts_lines), each entry's window its own line.
 static int MatchStarts(const pire_gpu_scanner* rsc, const uint8_t* d_corpus, const uint64_t* d_offsets, uint64_t fixed_len,
                        uint64_t n, const uint64_t* d_pos, uint64_t base, uint32_t flags, uint64_t max_back,
                        const uint32_t* d_strings, const uint64_t* d_ends, const uint32_t* d_ids, const uint64_t* d_first,
-                       const uint64_t* d_found, uint64_t capacity, uint64_t* d_starts, uint8_t* d_open, void* stream)
+                       const uint64_t* d_found, uint64_t capacity, uint64_t* d_starts, uint8_t* d_open, void* stream,
+                       bool lines = false)
 {
     int rc = CheckRunnable(rsc);
     if (rc != PIRE_GPU_OK)
@@ -874,6 +913,7 @@ static int MatchStarts(const pire_gpu_scanner* rsc, const uint8_t* d_corpus, con
     a.ends_capacity = capacity;
     a.match_starts = d_starts;
     a.match_open = d_open;
+    a.trim = lines ? 1 : 0;
     CUDA_TRY(LaunchMatchStarts(a, rsc->device, static_cast<cudaStream_t>(stream)));
     return PIRE_GPU_OK;
 }
@@ -895,6 +935,20 @@ int pire_gpu_match_starts_batch(const pire_gpu_scanner* rsc, const uint8_t* d_co
 {
     return MatchStarts(rsc, d_corpus, d_offsets, fixed_len, n, d_pos, 0, flags, max_back, d_strings, d_ends, d_ids, d_first,
                        d_found, capacity, d_starts, d_open, stream);
+}
+
+int pire_gpu_match_starts_lines(const pire_gpu_scanner* rsc, const uint8_t* d_text, const uint64_t* d_line_offsets,
+                                uint64_t n_lines, uint32_t flags, uint64_t max_back, const uint32_t* d_lines,
+                                const uint64_t* d_ends, const uint32_t* d_ids, const uint64_t* d_first, const uint64_t* d_found,
+                                uint64_t capacity, uint64_t* d_starts, uint8_t* d_open, void* stream)
+{
+    int rc = CheckRunnable(rsc);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (!d_line_offsets || !d_lines)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_match_starts_lines needs the line offsets and d_lines");
+    return MatchStarts(rsc, d_text, d_line_offsets, 0, n_lines, nullptr, 0, flags & ~PIRE_GPU_RUN_LINES, max_back, d_lines,
+                       d_ends, d_ids, d_first, d_found, capacity, d_starts, d_open, stream, true);
 }
 
 int pire_gpu_scanner_tune(pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets,

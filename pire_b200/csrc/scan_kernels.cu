@@ -2230,6 +2230,50 @@ __device__ __forceinline__ void LoadBlock32(const uint8_t* aligned, uintptr_t bu
     }
 }
 
+// ScanTextKernel's segments of a text whose last separator sits at `total`, for `warps` warps, as MatchEndsTextKernel
+// takes them (ScanTextKernel spells the same arithmetic and search inline: through these helpers it compiled to other
+// code than the one its measurements are for).  Segment size: about kTextSegment bytes, chosen so that the units (32
+// segments) come out as a whole number of rounds over the grid's warps -- with a couple of units per warp, one unit more
+// or less is a third of the run time.
+struct TextSegments {
+    uint64_t seg;           // bytes per segment, a multiple of 32
+    uint64_t segments;
+    uint64_t units;         // groups of 32 segments, one warp's at a time
+};
+
+__device__ __forceinline__ TextSegments TextSegmentsOf(uint64_t total, uint32_t mis0, uint64_t warps)
+{
+    TextSegments g;
+    const uint64_t lanes = 32 * warps;
+    const uint64_t rounds = (total + 64 + lanes * kTextSegment - 1) / (lanes * kTextSegment);
+    uint64_t seg = ((total + 64 + lanes * rounds - 1) / (lanes * rounds) + 31) / 32 * 32;
+    g.seg = seg < 64 ? 64 : seg;
+    g.segments = (total + mis0) / g.seg + 1;
+    g.units = (g.segments + 31) / 32;
+    return g;
+}
+
+// The first line that starts in segment sidx, which ends at seg_hi: true, with the line and its start pos0, when there
+// is one.
+__device__ __forceinline__ bool TextFirstLine(const ScanArgs& a, uint64_t sidx, uint64_t seg, uint32_t mis0, uint64_t seg_hi,
+                                              uint64_t& line, uint64_t& pos0)
+{
+    const uint64_t seg_lo = sidx * seg > mis0 ? sidx * seg - mis0 : 0;
+    uint64_t lo = 0, hi = a.n;              // first line that starts at or behind seg_lo
+    while (lo < hi) {
+        const uint64_t mid = (lo + hi) >> 1;
+        if (a.offsets[mid] < seg_lo)
+            lo = mid + 1;
+        else
+            hi = mid;
+    }
+    if (lo >= a.n)
+        return false;
+    line = lo;
+    pos0 = a.offsets[lo];
+    return pos0 < seg_hi;
+}
+
 template <bool kPred>
 __global__ void __launch_bounds__(kBlock, kTextBlocksPerSM) ScanTextKernel(const __grid_constant__ ScanArgs a)
 {
@@ -3003,7 +3047,11 @@ __device__ __forceinline__ void PrefixCheck(const ScanArgs& a, uint32_t H, const
         l.stop = true;
 }
 
-__global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) MatchStartsKernel(const __grid_constant__ ScanArgs a)
+// The walk of MatchStartsKernel, and with kLines that of MatchStartsLinesKernel (pire_gpu_match_starts_lines): the
+// offsets are a text's lines, string i's window is line i itself, [offsets[i], offsets[i + 1] - 1), and positions are
+// the text's.  `a` by value, as the kernels take it: so MatchStartsKernel compiles to what it did when this was its body.
+template <bool kLines>
+__device__ __forceinline__ void MatchStartsWalk(const ScanArgs a)
 {
     uint8_t* const smem = pire_b200_smem;
     SharedView sv = CarveShared(smem, a.hot);
@@ -3034,7 +3082,7 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) MatchStartsKernel
     const uint32_t lane = threadIdx.x & 31;
     const uint32_t stage = SmemAddr(sv.stage) + (((threadIdx.x >> 5) * kStageSlots) * 32 + lane) * 16;
     const uintptr_t buf_lo = reinterpret_cast<uintptr_t>(a.corpus);
-    const uintptr_t buf_hi = buf_lo + (a.offsets ? a.offsets[a.n] : a.n * a.fixed_len);
+    const uintptr_t buf_hi = buf_lo + (a.offsets ? a.offsets[a.n] - (kLines ? 1 : 0) : a.n * a.fixed_len);
     const uint64_t first = a.entries_first ? *a.entries_first : 0;
     const uint64_t found = *a.entries_found;
     const uint64_t last = found < a.ends_capacity ? found : a.ends_capacity;
@@ -3061,13 +3109,13 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) MatchStartsKernel
                 uint64_t b, e;
                 if (a.offsets) {
                     b = a.offsets[si];
-                    e = a.offsets[si + 1];
+                    e = a.offsets[si + 1] - (kLines ? 1 : 0);
                     e = e < b ? b : e;
                 } else {
                     b = (uint64_t) si * a.fixed_len;
                     e = b + a.fixed_len;
                 }
-                wend = a.window_end ? a.window_end[si] : a.ends_base + (e - b);
+                wend = kLines ? e : a.window_end ? a.window_end[si] : a.ends_base + (e - b);
                 wstart = wend - (e - b);
                 valid = wend >= e - b && end >= wstart && end <= wend;    // entries outside the window are not ours
                 wbase = a.corpus + b;
@@ -3173,6 +3221,16 @@ __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) MatchStartsKernel
                 a.match_open[k] = open ? 1 : 0;
         }
     }
+}
+
+__global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) MatchStartsKernel(const __grid_constant__ ScanArgs a)
+{
+    MatchStartsWalk<false>(a);
+}
+
+__global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) MatchStartsLinesKernel(const __grid_constant__ ScanArgs a)
+{
+    MatchStartsWalk<true>(a);
 }
 
 // ---------------------------------------------------------------- counting (HalfFinalScanner)
@@ -3768,6 +3826,287 @@ template <bool kWrite>
 __global__ void __launch_bounds__(kBlock, kGenericBlocksPerSM) MatchEndsBatchKernel(const __grid_constant__ ScanArgs a)
 {
     CountWalk<0, false, true, EndsSink<kWrite>>(a);
+}
+
+// ---------------------------------------------------------------- where the matches end in the lines of a text
+//
+// pire_gpu_match_ends_lines: every line its own HalfFinalScanner run, walked where the lines lie.  ScanTextKernel's
+// segments (a lane owns the lines that start in its segment and runs past its end to finish the last of them; the hot
+// rows' '\n' leads to the start state, so the walk restarts behind a line by itself) with CountWalk's sink:
+//   * a 16-byte chunk without a newline goes through SinkChunk16: one running maximum tells whether it entered a final
+//     state (final hot states carry the highest ids);
+//   * a chunk with newlines is walked the same way with the states in front of its bytes packed as ScanTextKernel packs
+//     them; when it entered no final state, each '\n' takes the line's EndMark step (with END) from its packed state,
+//     reports the line's match bit and state, and takes the next line's Initialize and BeginMark actions -- the only
+//     entries such a chunk can have.  The counting walk also takes a chunk with final states this way when it stays in
+//     the hot rows, adding the list lengths of the states entered in a second pass;
+//   * the rest (a final state or the sink on the way, the unaligned start of a lane's first line) byte by byte.
+// Two launches around a scan, as in LaunchMatchEndsBatch.  The counting walk reports every line's match bit and state,
+// and leaves each lane's number of entries at entry_counts[first line + 1] (the rest zeroed by the caller) and the first
+// of its lines with an entry at last_states[first line].  The writing walk starts there, from entry_first[first line],
+// and stops at the lane's last entry (or the capacity): lanes without entries walk nothing.  A lane's lines are
+// consecutive, so the layout is line order.
+constexpr uint32_t kNoLine = 0xFFFFFFFFu;
+constexpr uint32_t kLinesPackOffset = 1024;          // behind the hot states' list lengths (at most 255 words)
+// the counting walk, behind the packed states: the hot states' reports, then the list lengths of the states their
+// EndMark step enters (0 for the non-final ones)
+constexpr uint32_t kLinesFinOffset = kLinesPackOffset + kBlock * 16;
+constexpr uint32_t kLinesEndOffset = kLinesFinOffset + 256 * sizeof(DeviceFin);
+constexpr size_t kLinesSharedBytes = kLinesEndOffset + 256 * 4;
+
+struct LinesLane {
+    uint32_t line;          // the line being walked
+    uint32_t hit;           // counting walk: the first line with an entry, kNoLine before it
+    bool active;            // false: no line of this lane is left (or, writing, no entry)
+};
+
+// after a TakeAction of line c.line that wrote o.n - n0 entries (writing: their line) or counted them (the first line with
+// an entry)
+template <bool kWrite>
+__device__ __forceinline__ void LineEntries(const ScanArgs& a, const EndsSink<kWrite>& o, LinesLane& c, uint64_t n0)
+{
+    if (kWrite) {
+        if (a.strings)
+            for (uint64_t k = n0; k < o.n; ++k)
+                a.strings[k] = c.line;
+    } else if (o.n != n0 && c.hit == kNoLine) {
+        c.hit = c.line;
+    }
+}
+
+template <bool kWrite>
+__device__ __forceinline__ void LineTake(const ScanArgs& a, const Tables& t, EndsSink<kWrite>& o, LinesLane& c, uint32_t s, uint64_t pos)
+{
+    const uint64_t n0 = o.n;
+    SinkTake(a, t, o, s, pos);
+    LineEntries(a, o, c, n0);
+}
+
+// Initialize()'s and (with BEGIN) BeginMark's TakeAction at the start of a line
+template <bool kWrite>
+__device__ __forceinline__ void LineBegin(const ScanArgs& a, const Tables& t, EndsSink<kWrite>& o, LinesLane& c, uint64_t pos)
+{
+    LineTake(a, t, o, c, a.initial, pos);
+    if (a.with_begin)
+        LineTake(a, t, o, c, a.start, pos);
+}
+
+// The '\n' at text position `at` ends line c.line, whose state in front of it is `st`: its EndMark step, its report
+// (counting walk), the next line's start.  False when the lane has no line left.  The counting walk takes a hot state's
+// EndMark entries and report from shared memory (`fin_hot`, `end_len`).
+template <bool kWrite>
+__device__ __forceinline__ bool LineEnd(const ScanArgs& a, const Tables& t, uint32_t outs, EndsSink<kWrite>& o, LinesLane& c, uint32_t st,
+                                        uint64_t at, uint64_t seg_hi, const DeviceFin* fin_hot, const uint32_t* end_len)
+{
+    if (a.through_end) {                                                // Step(EndMark)
+        if (!kWrite && st < t.H) {
+            o.n += end_len[st];
+            if (end_len[st] != 0 && c.hit == kNoLine)
+                c.hit = c.line;
+        } else {
+            LineTake(a, t, o, c, FullNext(t, st, a.end_class), at);
+        }
+    }
+    if (!kWrite)
+        TextReport(a, outs, c.line, st < t.H ? fin_hot[st] : a.fin[st]);
+    ++c.line;
+    if (c.line >= a.n || at + 1 >= seg_hi) {                          // the next line starts behind the segment
+        c.active = false;
+        return false;
+    }
+    LineBegin(a, t, o, c, at + 1);
+    return true;
+}
+
+// Bytes [from, 16) of the chunk v at text position cpos, one by one from the complete state `full`; returns the state
+// behind them.
+template <bool kWrite>
+__device__ __forceinline__ uint32_t LinesSlow(const ScanArgs& a, const Tables& t, uint32_t outs, EndsSink<kWrite>& o, LinesLane& c,
+                                              uint32_t full, uint4 v, int64_t cpos, uint32_t from, uint64_t seg_hi,
+                                              const DeviceFin* fin_hot, const uint32_t* end_len)
+{
+    EdgeBytes eb(v, from);
+    for (uint32_t j = from; j < 16; ++j) {
+        const uint32_t b = eb.Next();
+        const uint64_t at = (uint64_t) (cpos + (int64_t) j);
+        if (b == '\n') {
+            if (!LineEnd(a, t, outs, o, c, full, at, seg_hi, fin_hot, end_len))
+                break;
+            full = a.start;
+            continue;
+        }
+        full = SlowStep(t, full, b);
+        LineTake(a, t, o, c, full, at + 1);
+    }
+    return full;
+}
+
+// Four steps, q collecting the state in front of each byte (TextWord) and top the highest state entered.
+__device__ __forceinline__ void LinesWord(const Tables& t, uint32_t& g, uint32_t w, uint32_t& q, uint32_t& top)
+{
+#pragma unroll
+    for (uint32_t i = 0; i < 4; ++i) {
+        asm("mad.lo.u32 %0, %0, 256, %1;" : "+r"(q) : "r"(g));       // q = q << 8 | g, on the FMA pipe
+        FastStep<false>(t, g, w, 0x5540u + i);
+        top = max(top, g);
+    }
+}
+
+template <bool kWrite>
+__device__ __forceinline__ void LinesChunk16(const ScanArgs& a, const Tables& t, const uint32_t* hot_len, uint32_t outs, LinesLane& c,
+                                             LaneState& s, EndsSink<kWrite>& o, uint4 v, int64_t cpos, uint32_t from, uint64_t seg_hi,
+                                             uint32_t packs, const DeviceFin* fin_hot, const uint32_t* end_len)
+{
+    if (!c.active || from >= 16)
+        return;
+    uint32_t nl = NewlineNibble(v.x) | (NewlineNibble(v.y) << 4) | (NewlineNibble(v.z) << 8) | (NewlineNibble(v.w) << 12);
+    bool done = false;
+    if (from == 0 && nl == 0) {
+        const uint64_t n0 = o.n;
+        SinkChunk16<0, false>(a, t, hot_len, s, v, (uint64_t) cpos, o);
+        LineEntries(a, o, c, n0);
+        done = true;
+    } else if (from == 0) {
+        uint32_t g = s.g, top = 0;
+        uint4 q = make_uint4(0, 0, 0, 0);
+        LinesWord(t, g, v.x, q.x, top);
+        LinesWord(t, g, v.y, q.y, top);
+        LinesWord(t, g, v.z, q.z, top);
+        LinesWord(t, g, v.w, q.w, top);
+        // counting, a chunk that stays in the hot rows and ends none of the lane's lines for good: the list lengths of
+        // the states entered, less those of the start states behind the '\n's (not TakeActions of the walk)
+        const bool sum = !kWrite && top >= a.first_final_hot && top < t.H && cpos + 16 < (int64_t) seg_hi
+                         && c.line + (uint32_t) __popc(nl) < a.n;
+        if (sum) {
+            uint32_t add = 0;
+            g = s.g;
+#pragma unroll
+            for (int w = 0; w < 4; ++w) {
+                const uint32_t word = w == 0 ? v.x : w == 1 ? v.y : w == 2 ? v.z : v.w;
+#pragma unroll
+                for (int b = 0; b < 4; ++b) {
+                    FastStep<false>(t, g, word, 0x5540 + b);
+                    add += hot_len[g];
+                }
+            }
+            add -= (uint32_t) __popc(nl) * hot_len[a.start];
+            if (add != 0 && c.hit == kNoLine)
+                c.hit = c.line;                 // the chunk's first line: at or before the first with an entry
+            o.n += add;
+        }
+        if (top < a.first_final_hot || sum) {   // else a final state or the sink (the highest id) on the way
+            s.g = g;
+            asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(packs), "r"(q.x), "r"(q.y), "r"(q.z), "r"(q.w) : "memory");
+            do {
+                const uint32_t k = (uint32_t) __ffs((int) nl) - 1u;
+                nl &= nl - 1u;
+                uint32_t st;        // the state in front of byte k: byte 3 - k % 4 of word k / 4
+                asm volatile("ld.shared.u8 %0, [%1];" : "=r"(st) : "r"(packs + (k ^ 3u)) : "memory");
+                if (!LineEnd(a, t, outs, o, c, st, (uint64_t) (cpos + (int64_t) k), seg_hi, fin_hot, end_len))
+                    break;
+            } while (nl);
+            done = true;
+        }
+    }
+    if (!done)
+        SetFull(t, s, LinesSlow(a, t, outs, o, c, FullState(t, s), v, cpos, from, seg_hi, fin_hot, end_len));
+    if (kWrite && o.Full())                 // the lane's last entry (or the capacity) is behind it
+        c.active = false;
+}
+
+template <bool kWrite>
+__global__ void __launch_bounds__(kBlock, kTextBlocksPerSM) MatchEndsTextKernel(const __grid_constant__ ScanArgs a)
+{
+    uint8_t* const smem = pire_b200_smem;
+    SharedView sv = CarveShared(smem, a.hot);
+    StageTables(a, sv, a.hot8, a.hot);
+    for (uint32_t g = threadIdx.x; g < a.hot; g += blockDim.x)
+        sv.hot[g * kHotStride + '\n'] = (uint8_t) a.start;
+    // the counting walk: the accept-list length of every hot state (0 for the non-final ones)
+    uint32_t* const hot_len = reinterpret_cast<uint32_t*>(sv.stage);
+    DeviceFin* const fin_hot = reinterpret_cast<DeviceFin*>(sv.stage + kLinesFinOffset);
+    uint32_t* const end_len = reinterpret_cast<uint32_t*>(sv.stage + kLinesEndOffset);
+    Tables t;
+    t.hot = sv.hot;
+    t.base = SmemAddr(sv.hot);
+    t.cls = sv.cls;
+    t.full = a.full;
+    t.H = a.hot;
+    t.letters = a.letters;
+    t.wide = a.wide;
+    t.m0 = 0;
+    if (!kWrite)
+        for (uint32_t i = threadIdx.x; i < a.hot; i += blockDim.x) {
+            hot_len[i] = i >= a.first_final_hot ? __ldg(a.acc_begin + i + 1) - __ldg(a.acc_begin + i) : 0u;
+            fin_hot[i] = a.fin[i];
+            const uint32_t e = FullNext(t, i, a.end_class);
+            end_len[i] = (__ldg(a.flags + e) & 1u) ? __ldg(a.acc_begin + e + 1) - __ldg(a.acc_begin + e) : 0u;
+        }
+    __syncthreads();
+
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t outs = kWrite ? 0u : TextOutputs(a);
+    const uint32_t packs = SmemAddr(sv.stage) + kLinesPackOffset + threadIdx.x * 16u;
+    const uint64_t total = a.offsets[a.n] - 1;           // position of the last separator (real or the end of the text)
+    const uintptr_t buf_lo = reinterpret_cast<uintptr_t>(a.corpus);
+    const uintptr_t buf_hi = buf_lo + total;
+    const uint32_t mis0 = (uint32_t) (buf_lo & 31);
+    const uint64_t warps = (uint64_t) gridDim.x * kWarpsPerBlock;
+    const TextSegments segs = TextSegmentsOf(total, mis0, warps);
+
+    for (uint64_t unit = (uint64_t) blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5); unit < segs.units; unit += warps) {
+        const uint64_t sidx = unit * 32 + lane;
+        const uint64_t seg_hi = (sidx + 1) * segs.seg - mis0;
+        LinesLane c;
+        c.line = 0;
+        c.hit = kNoLine;
+        c.active = false;
+        EndsSink<kWrite> o;
+        o.n = o.stop = 0;
+        uint64_t first = 0, pos0 = 0;
+        if (sidx < segs.segments && TextFirstLine(a, sidx, segs.seg, mis0, seg_hi, first, pos0)) {
+            c.line = (uint32_t) first;
+            c.active = true;
+            if (kWrite) {
+                // from the first line with an entry to the last entry, cut at the capacity
+                const uint64_t to = a.entry_first[first] + a.entry_counts[first + 1];
+                o.n = a.entry_first[first];
+                o.stop = to < a.ends_capacity ? to : a.ends_capacity;
+                c.active = o.n < o.stop;
+                if (c.active) {
+                    c.line = a.last_states[first];
+                    pos0 = a.offsets[c.line];
+                }
+            }
+            if (c.active)
+                LineBegin(a, t, o, c, pos0);
+        }
+        const bool owner = !kWrite && c.active;
+        LaneState s;
+        SetFull(t, s, a.start);
+        int64_t cpos = (int64_t) ((pos0 + mis0) & ~31ull) - (int64_t) mis0;        // the 32-byte block the line starts in
+        uint32_t from = (uint32_t) ((int64_t) pos0 - cpos);
+        const uint8_t* p = a.corpus + cpos;
+        uint4 v0 = make_uint4(0, 0, 0, 0), v1 = v0;
+        if (c.active)
+            LoadBlock32(p, buf_lo, buf_hi, v0, v1);
+        while (__any_sync(0xffffffffu, c.active)) {
+            uint4 n0 = make_uint4(0, 0, 0, 0), n1 = n0;
+            if (c.active)
+                LoadBlock32(p + 32, buf_lo, buf_hi, n0, n1);
+            LinesChunk16(a, t, hot_len, outs, c, s, o, v0, cpos, from, seg_hi, packs, fin_hot, end_len);
+            LinesChunk16(a, t, hot_len, outs, c, s, o, v1, cpos + 16, from > 16 ? from - 16 : 0, seg_hi, packs, fin_hot, end_len);
+            from = 0;
+            v0 = n0;
+            v1 = n1;
+            p += 32;
+            cpos += 32;
+        }
+        if (owner) {
+            a.entry_counts[first + 1] = o.n;
+            a.last_states[first] = c.hit;
+        }
+    }
 }
 
 // ---------------------------------------------------------------- counting one string over the whole grid
@@ -4737,6 +5076,84 @@ cudaError_t LaunchMatchEndsBatch(const ScanArgs& a, int device, cudaStream_t str
     return err;
 }
 
+// Lines of a text (pire_gpu_match_ends_lines); the caller zeroes a.match_bits.  In stream (MatchEndsTextKernel) when the
+// start state is a hot row: the counting walk reports the lines and leaves each lane's total at entry_counts[its first
+// line + 1] of a zeroed array of n + 1 words whose word 0 is *a.found, their inclusive sum places every lane's lines, the
+// writing walk fills them in.  Otherwise -- no hot rows, or a hot set cut short of the start -- one line per lane: LaunchMatchEndsBatch over
+// the lines as a trimmed CSR batch, each line's positions from its offset on.
+cudaError_t LaunchMatchEndsLines(const ScanArgs& a, int device, cudaStream_t stream)
+{
+    if (a.n == 0)
+        return cudaSuccess;
+    if (a.start >= a.hot) {
+        ScanArgs lines = a;
+        cudaError_t err = ScratchAlloc(reinterpret_cast<void**>(&lines.pos), a.n * 8, stream);
+        if (err != cudaSuccess)
+            return err;
+        err = cudaMemcpyAsync(lines.pos, a.offsets, a.n * 8, cudaMemcpyDeviceToDevice, stream);
+        if (err == cudaSuccess)
+            err = LaunchMatchEndsBatch(lines, device, stream);
+        cudaFreeAsync(lines.pos, stream);
+        return err;
+    }
+    const void* count = reinterpret_cast<const void*>(&MatchEndsTextKernel<false>);
+    const void* emit = reinterpret_cast<const void*>(&MatchEndsTextKernel<true>);
+    // + the hot states' list lengths, each thread's packed states of a chunk, the hot states' reports and EndMark lengths
+    const size_t shared = ScanSharedBytes(a.hot, 0) + kLinesSharedBytes;
+    int optin = 0, sms = 0, per_sm = 0;
+    cudaError_t err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+    if (err == cudaSuccess)
+        err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err == cudaSuccess)
+        err = cudaFuncSetAttribute(count, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+    if (err == cudaSuccess)
+        err = cudaFuncSetAttribute(emit, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+    if (err == cudaSuccess)
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, count, kBlock, shared);
+    if (err != cudaSuccess)
+        return err;
+    if (per_sm < 1)
+        return cudaErrorLaunchOutOfResources;
+    const uint64_t items = a.n + 1;
+    unsigned long long *counts = nullptr, *first = nullptr;
+    void* temp = nullptr;
+    size_t temp_bytes = 0;
+    err = cub::DeviceScan::InclusiveSum(nullptr, temp_bytes, counts, first, items, stream);
+    if (err == cudaSuccess) err = ScratchAlloc(reinterpret_cast<void**>(&counts), items * 8, stream);
+    if (err == cudaSuccess) err = ScratchAlloc(reinterpret_cast<void**>(&first), items * 8, stream);
+    uint32_t* lines = nullptr;
+    if (err == cudaSuccess) err = ScratchAlloc(&temp, temp_bytes, stream);
+    if (err == cudaSuccess) err = ScratchAlloc(reinterpret_cast<void**>(&lines), a.n * 4, stream);
+    if (err == cudaSuccess) err = cudaMemsetAsync(counts, 0, items * 8, stream);
+    if (err == cudaSuccess) err = cudaMemcpyAsync(counts, a.found, 8, cudaMemcpyDeviceToDevice, stream);
+    ScanArgs walk = a;
+    walk.entry_counts = counts;
+    walk.entry_first = first;
+    walk.last_states = lines;
+    void* args[] = {&walk};
+    // the persistent grid whole, as in LaunchLines: the number of segments depends on the text's size (offsets[n])
+    const dim3 grid((unsigned) (sms * per_sm));
+    if (err == cudaSuccess) {
+        err = cudaLaunchKernel(count, grid, dim3(kBlock), args, shared, stream);
+        if (err == cudaSuccess)
+            g_launches.fetch_add(1, std::memory_order_relaxed);
+    }
+    if (err == cudaSuccess)
+        err = cub::DeviceScan::InclusiveSum(temp, temp_bytes, counts, first, items, stream);
+    if (err == cudaSuccess) {
+        err = cudaLaunchKernel(emit, grid, dim3(kBlock), args, shared, stream);
+        if (err == cudaSuccess)
+            g_launches.fetch_add(1, std::memory_order_relaxed);
+    }
+    if (err == cudaSuccess)
+        err = cudaMemcpyAsync(a.found, first + a.n, 8, cudaMemcpyDeviceToDevice, stream);
+    if (counts) cudaFreeAsync(counts, stream);
+    if (first) cudaFreeAsync(first, stream);
+    if (temp) cudaFreeAsync(temp, stream);
+    if (lines) cudaFreeAsync(lines, stream);
+    return err;
+}
+
 cudaError_t LaunchVisitCount(const ScanArgs& a, cudaStream_t stream)
 {
     if (a.n == 0)
@@ -4775,7 +5192,7 @@ __global__ void __launch_bounds__(256) LengthKeysKernel(const uint64_t* __restri
 // masks (256 words) and, up to kStartsHotLiveWords words a row, their live rows.
 cudaError_t LaunchMatchStarts(const ScanArgs& a, int device, cudaStream_t stream)
 {
-    const void* fn = reinterpret_cast<const void*>(&MatchStartsKernel);
+    const void* fn = a.trim ? reinterpret_cast<const void*>(&MatchStartsLinesKernel) : reinterpret_cast<const void*>(&MatchStartsKernel);
     int optin = 0, sms = 0;
     cudaError_t err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
     if (err == cudaSuccess)

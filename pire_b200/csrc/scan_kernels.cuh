@@ -95,7 +95,9 @@ struct ScanArgs {
     uint64_t* pos;               // n words: each string's first position, advanced by its length; or null (all 0)
     unsigned long long* entry_counts;      // scratch, n + 1: *found as the call found it, then each string's entries
     const unsigned long long* entry_first; // scratch, n + 1: the inclusive sum of entry_counts
-    uint32_t* last_states;       // scratch, n: each string's state before EndMark, new numbering (0xFFFFFFFF: unknown start)
+    uint32_t* last_states;       // scratch, n: each string's state before EndMark, new numbering (0xFFFFFFFF: unknown start);
+                                 // lines of a text (pire_gpu_match_ends_lines): a lane's first line with an entry, at the
+                                 // index of its first line (entry_counts / entry_first: the lane's total there)
     // where the matches start (pire_gpu_match_starts_*): entries [*entries_first, min(*entries_found, ends_capacity)) of
     // entry_strings / entry_ends / entry_ids; string i's window is [w - len_i, w) with w = window_end[i], or ends_base +
     // len_i when that is null.  An entry's walk goes left from its end to the window start (or max_back bytes), with
@@ -169,8 +171,13 @@ cudaError_t LaunchCount(const ScanArgs& a, int device, cudaStream_t stream, bool
 // `from`, string i's entries from index *a.found + (the entries of strings 0..i-1) on, placed by a scan over the strings;
 // then match bits, states and a.pos as LaunchCount's, and *a.found advanced by the call's total
 cudaError_t LaunchMatchEndsBatch(const ScanArgs& a, int device, cudaStream_t stream);
+// Every TakeAction of HalfFinalScanner on each line of a text (a.offsets from SplitLines, a.trim 1), line l from
+// Initialize() with its positions from offsets[l] on: LaunchMatchEndsBatch's layout in line order, match bits (OR-ed into
+// a zeroed bitmap) and states as LaunchLines gives them, *a.found advanced by the call's total
+cudaError_t LaunchMatchEndsLines(const ScanArgs& a, int device, cudaStream_t stream);
 // The leftmost start of every match-ends entry (MatchStartsKernel): one entry per lane, walked leftwards through a
-// reversed scanner from its end, groups of 32 entries handed to warps of a persistent grid
+// reversed scanner from its end, groups of 32 entries handed to warps of a persistent grid.  a.trim 1: the offsets are a
+// text's lines and each entry's window is its own line (MatchStartsLinesKernel)
 cudaError_t LaunchMatchStarts(const ScanArgs& a, int device, cudaStream_t stream);
 // d_order <- string indices, longest half-octave length bucket first, corpus order inside a bucket (stable CUB radix sort).
 // stream-ordered scratch from the library's own per-device pool (see scan_kernels.cu)

@@ -948,6 +948,130 @@ class BatchMatchEnds:
         return self.StateTensor().cpu().numpy().view(np.uint32)
 
 
+class LineMatchEnds:
+    """Where the matches end in every line of a text (pire_gpu_match_ends_lines): each line of a ``Batch.from_text``
+    batch is its own run, as ``Runner(sc).Begin().Run(line).End()`` runs it, and yields one entry (line, end, regexp id)
+    for every TakeAction, ordered by line, then in walk order within a line.  Ends are positions in the text: byte k of
+    line l ends at offsets[l] + k + 1, Initialize() and BeginMark at offsets[l], EndMark at offsets[l + 1] - 1.  The
+    entries go to device tensors of ``capacity`` entries; ``FoundTensor()`` counts all of them, even past the capacity,
+    whose entries are dropped.  ``Begin()`` / ``End()`` choose the marks of every line; the one launch happens at the first
+    result, so that ``End()`` folds into it.  ``LinesTensor()``, ``EndsTensor()``, ``IdsTensor()``, ``FoundTensor()`` and
+    ``StateTensor()`` do not synchronise; ``Found()``, ``Lines()``, ``Ends()``, ``Ids()``, ``Matches()`` and ``States()``
+    do."""
+
+    def __init__(self, sc, capacity):
+        torch = _torch()
+        self.Sc = sc
+        self.capacity = int(capacity)
+        dev = torch.device("cuda", sc.device)
+        self._lines = torch.empty(self.capacity, dtype=torch.int32, device=dev)
+        self._ends = torch.empty(self.capacity, dtype=torch.int64, device=dev)
+        self._ids = torch.empty(self.capacity, dtype=torch.int32, device=dev)
+        self._found = torch.zeros(1, dtype=torch.int64, device=dev)
+        self._flags = 0
+        self.batch = None
+        self.n = 0
+        self._ran = False
+
+    def Begin(self):
+        if self.batch is not None:
+            raise ValueError("Begin() must precede Run()")
+        self._flags |= N.RUN_BEGIN
+        return self
+
+    def Run(self, batch):
+        if not batch.trim or batch.offsets is None:
+            raise ValueError("LineMatchEnds.Run takes a line batch (Batch.from_text)")
+        if batch.order is not None:
+            raise ValueError("LineMatchEnds takes no length-ordered batch")
+        if self.batch is not None:
+            raise ValueError("LineMatchEnds runs one text")
+        if batch.device != self._found.device:
+            raise ValueError("the batch must be on the scanner's device")
+        torch = _torch()
+        self.batch = batch
+        self.n = batch.n
+        self._states = torch.empty(self.n, dtype=torch.int32, device=self._found.device)
+        self._bits = torch.empty((self.n + 31) // 32, dtype=torch.int32, device=self._found.device)
+        return self
+
+    def End(self):
+        if self._ran:
+            raise ValueError("End() must precede the first result")
+        self._flags |= N.RUN_END
+        return self
+
+    def _ensure(self):
+        if self._ran:
+            return
+        if self.batch is None:
+            raise ValueError("LineMatchEnds needs Run(batch) first")
+        torch = _torch()
+        b = self.batch
+        stream = torch.cuda.current_stream(self._found.device).cuda_stream
+        N.check(N.lib.pire_gpu_match_ends_lines(self.Sc._h, b.corpus.data_ptr(), b.offsets.data_ptr(), self.n, self._flags,
+                                                self._lines.data_ptr(), self._ends.data_ptr(), self._ids.data_ptr(),
+                                                self.capacity, self._found.data_ptr(), self._bits.data_ptr(),
+                                                self._states.data_ptr(), stream), "pire_gpu_match_ends_lines")
+        self._ran = True
+
+    # without a synchronise ------------------------------------------------------------
+    def LinesTensor(self):
+        """The device tensor of line indices (int32 holding u32), ``capacity`` long."""
+        self._ensure()
+        return self._lines
+
+    def EndsTensor(self):
+        """The device tensor of ends (int64 holding u64, text positions), ``capacity`` long."""
+        self._ensure()
+        return self._ends
+
+    def IdsTensor(self):
+        """The device tensor of regexp ids (int32 holding u32), ``capacity`` long."""
+        self._ensure()
+        return self._ids
+
+    def FoundTensor(self):
+        """The device word (int64 holding u64) counting every entry, also those past the capacity."""
+        self._ensure()
+        return self._found
+
+    def StateTensor(self):
+        """The device tensor (int32, one per line) of each line's last state, reference numbering."""
+        self._ensure()
+        return self._states
+
+    # synchronising --------------------------------------------------------------------
+    def Found(self):
+        """The number of entries, also those past the capacity."""
+        return int(self.FoundTensor().item())
+
+    def Lines(self):
+        """The first min(Found(), capacity) line indices, as numpy u32."""
+        k = min(self.Found(), self.capacity)
+        return self._lines[:k].cpu().numpy().view(np.uint32)
+
+    def Ends(self):
+        """The first min(Found(), capacity) ends, as numpy u64."""
+        k = min(self.Found(), self.capacity)
+        return self._ends[:k].cpu().numpy().view(np.uint64)
+
+    def Ids(self):
+        """The first min(Found(), capacity) regexp ids, as numpy u32."""
+        k = min(self.Found(), self.capacity)
+        return self._ids[:k].cpu().numpy().view(np.uint32)
+
+    def Matches(self):
+        """numpy bool[lines]: Final() of each line's state, as Runner gives it for the line batch."""
+        self._ensure()
+        words = self._bits.cpu().numpy().view(np.uint32)
+        return np.unpackbits(words.view(np.uint8), bitorder="little")[: self.n].astype(bool)
+
+    def States(self):
+        """StateIndex() of each line's state (reference numbering)."""
+        return self.StateTensor().cpu().numpy().view(np.uint32)
+
+
 NO_START = 0xFFFFFFFFFFFFFFFF
 
 
@@ -983,14 +1107,15 @@ def MatchStarts(rsc, ends, window, base=0, begin=True, end=True, max_back=0):
     """Where the matches ``ends`` lists start (pire_gpu_match_starts_string / _batch): Pire::LongestSuffix through
     ``rsc``, a Scanner of the same patterns built with Fsm::Reverse() (glued in the same order), walked leftwards from
     each entry's end and testing the entry's regexp id.  ``ends`` is a ``StringMatchEnds`` whose window is a uint8 CUDA
-    tensor holding the text bytes at positions [base, base + numel), or a ``BatchMatchEnds`` whose window is the
-    ``Batch`` of its last round (each stream's window ends where ``PosTensor()`` says).  ``begin`` says that the window
+    tensor holding the text bytes at positions [base, base + numel), a ``BatchMatchEnds`` whose window is the
+    ``Batch`` of its last round (each stream's window ends where ``PosTensor()`` says), or a ``LineMatchEnds`` whose
+    window is its line batch (each entry's window is its own line, pire_gpu_match_starts_lines).  ``begin`` says that the window
     starts where the text begins (BeginMark), ``end`` that the text ended with End() (EndMark); ``max_back`` > 0 bounds
     every walk.  Entries outside the window are left as NO_START.  Launches on the current stream, no synchronise."""
     torch = _torch()
     flags = (N.RUN_BEGIN if begin else 0) | (N.RUN_END if end else 0)
-    if not isinstance(ends, (StringMatchEnds, BatchMatchEnds)):
-        raise TypeError("ends must be a StringMatchEnds or a BatchMatchEnds")
+    if not isinstance(ends, (StringMatchEnds, BatchMatchEnds, LineMatchEnds)):
+        raise TypeError("ends must be a StringMatchEnds, a BatchMatchEnds or a LineMatchEnds")
     dev = ends.EndsTensor().device
     starts = torch.full((ends.capacity,), -1, dtype=torch.int64, device=dev)
     open_ = torch.zeros(ends.capacity, dtype=torch.uint8, device=dev)
@@ -1004,6 +1129,14 @@ def MatchStarts(rsc, ends, window, base=0, begin=True, end=True, max_back=0):
                                                    ends.EndsTensor().data_ptr(), ends.IdsTensor().data_ptr(), None,
                                                    ends.FoundTensor().data_ptr(), ends.capacity, starts.data_ptr(),
                                                    open_.data_ptr(), stream), "pire_gpu_match_starts_string")
+    elif isinstance(ends, LineMatchEnds):
+        if not window.trim or window.order is not None or window.n != ends.n or window.device != dev:
+            raise ValueError("window must be the line batch of the ends")
+        N.check(N.lib.pire_gpu_match_starts_lines(rsc._h, window.corpus.data_ptr(), window.offsets.data_ptr(), window.n,
+                                                  flags, int(max_back), ends.LinesTensor().data_ptr(),
+                                                  ends.EndsTensor().data_ptr(), ends.IdsTensor().data_ptr(), None,
+                                                  ends.FoundTensor().data_ptr(), ends.capacity, starts.data_ptr(),
+                                                  open_.data_ptr(), stream), "pire_gpu_match_starts_lines")
     else:
         if window.trim or window.order is not None or window.n != ends.n or window.device != dev:
             raise ValueError("window must be a plain batch of the ends' n streams on the scanner's device")

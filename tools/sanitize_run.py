@@ -293,5 +293,17 @@ assert (part.Ends() == full.Ends()[: total // 2]).all() and (part.Strings() == f
 key = full.Strings().astype(np.int64) * regs + full.Ids()
 assert (np.bincount(key, minlength=len(strings) * regs).reshape(-1, regs) == c.Counts().cpu().numpy()).all()
 print("ok match_ends_batch_from", flush=True)
+# where the matches end in every line of a text (pire_gpu_match_ends_lines): the ragged strings above joined into a text,
+# into a buffer too small for the answer and one with room for all of it, against count_batch with LINES
+text = torch.frombuffer(bytearray(b"\n".join(s.replace(b"\n", b" ") for s in strings)), dtype=torch.uint8).to("cuda:0")
+lb = P.Batch.from_text(text)
+lc = P.HalfFinalCount(sc, lb)
+ltotal = int(lc.counts.sum())
+lfull = P.LineMatchEnds(sc, ltotal).Begin().Run(lb).End()
+lpart = P.LineMatchEnds(sc, ltotal // 2).Begin().Run(lb).End()
+assert lfull.Found() == lpart.Found() == ltotal and (lpart.Ends() == lfull.Ends()[: ltotal // 2]).all()
+key = lfull.Lines().astype(np.int64) * regs + lfull.Ids()
+assert (np.bincount(key, minlength=lb.n * regs).reshape(-1, regs) == lc.counts).all()
+print("ok match_ends_lines", flush=True)
 torch.cuda.synchronize()
 print("sanitize_run done, launches:", N.lib.pire_gpu_launch_count())
