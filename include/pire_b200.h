@@ -542,6 +542,55 @@ int pire_gpu_run_batch_host(const pire_gpu_scanner* sc,
                             uint64_t fixed_len, uint64_t n, uint32_t flags,
                             uint32_t* match_bits, uint32_t* accept_masks, uint32_t* state_idx);
 
+/* A text of any size, from host memory, as device frames of whole lines (std::getline's loop of
+ * samples/pigrep/pigrep.cpp:15-21 over a stream that never has to fit in HBM).  The caller hands over the text's
+ * bytes in pieces of any size, split anywhere (read() blocks, an mmap'd file, a pinned buffer); every feed copies
+ * as many of them as fit into the next of three device slots, behind the line carried over from the slot before,
+ * and returns one frame: the slot's complete lines with the offsets pire_gpu_split_lines makes for them.
+ *   Feeding  *consumed receives the number of bytes taken from `bytes`; the caller calls again with the rest.  A
+ *            frame may have n_lines == 0 (no newline has arrived yet; its first offset word is 0).  With `last` set
+ *            and every byte consumed, the open line becomes the text's last line (no newline, as split_lines keeps
+ *            it) and the stream is finished: a later feed is PIRE_GPU_EINVAL.  An empty text has no lines; a text
+ *            ending in '\n' has no extra empty line.
+ *   Frames   lines are split_lines' lines of the whole text.  Shift a frame's offsets by first_byte and its line
+ *            numbers by first_line: the frames in order give split_lines over the concatenated text word for word
+ *            (frame k's last offset is frame k + 1's first one).  So a frame is accepted as it is by every call that
+ *            takes split_lines offsets: pire_gpu_run_lines, pire_gpu_count_batch with PIRE_GPU_RUN_LINES,
+ *            pire_gpu_match_ends_lines and pire_gpu_match_starts_lines.  The bytes behind a frame's last '\n' are
+ *            carried to the head of the next slot by a device-to-device copy, never sent again from the host.
+ *   Long lines  a line that does not fit in a slot grows the slot (at least doubling the room, so a long line is
+ *            copied device-to-device O(1) times per byte); only a line larger than free device memory fails
+ *            (PIRE_GPU_ECUDA with the CUDA message).  slot_bytes == 0 picks 256 MiB, the fastest of 16, 64 and 256 MiB
+ *            in tools/line_stream_bench.py (DESIGN.md 4); the device then holds about 0.8 GiB of slots and offsets.
+ *   Ordering  the bytes are copied and the lines found on the stream object's own stream, so the copy of frame
+ *            k + 1 overlaps the caller's work on frame k.  Everything a frame needs is in place for work the caller
+ *            enqueues on `stream` after feed returns.  The slot of frame k is written again by the feed that makes
+ *            frame k + 3; before writing it, that feed orders itself after the work that was enqueued on `stream`
+ *            when the feed making frame k + 1 was called.  So: work on frame k must be enqueued before the next feed
+ *            is called (on the `stream` passed to that feed), and the frame's buffers stay valid until it completes.
+ *            feed blocks until its own copies and the line split are done (split_lines synchronises) and until
+ *            the work on frame k - 3's slot has finished; it never waits for the work on frame k - 1.  When feed
+ *            returns, the caller's `bytes` are no longer referenced.
+ *   Input    pageable bytes are staged through the library's pinned buffers by its copy threads
+ *            (PIRE_B200_HOST_THREADS), pinned or cudaHostRegister-ed bytes are DMA-ed from the caller's buffer.
+ *   Errors   NULL bytes with n > 0, a NULL consumed or frame are PIRE_GPU_EINVAL; device < 0 or a device that does
+ *            not exist is PIRE_GPU_ENODEVICE at create.  A stream object belongs to one thread at a time.
+ * pire_gpu_line_stream_destroy synchronises the device (the caller's work on the last frames reads the slots) and
+ * frees the slots. */
+typedef struct pire_gpu_line_stream pire_gpu_line_stream;
+typedef struct pire_gpu_line_frame {
+    const uint8_t* d_text;            /* the frame's bytes on the device                                           */
+    const uint64_t* d_line_offsets;   /* n_lines + 1 words: what pire_gpu_split_lines makes for d_text, n_bytes    */
+    uint64_t n_lines;
+    uint64_t n_bytes;                 /* bytes of d_text (split_lines' n_bytes)                                    */
+    uint64_t first_line;              /* index in the whole text of the frame's line 0                             */
+    uint64_t first_byte;              /* offset in the whole text of d_text[0]                                     */
+} pire_gpu_line_frame;
+int pire_gpu_line_stream_create(int device, uint64_t slot_bytes, pire_gpu_line_stream** out);
+int pire_gpu_line_stream_feed(pire_gpu_line_stream* ls, const uint8_t* bytes, uint64_t n, int last, void* stream,
+                              uint64_t* consumed, pire_gpu_line_frame* frame);
+void pire_gpu_line_stream_destroy(pire_gpu_line_stream* ls);
+
 /* ---- several GPUs of one box ---------------------------------------------------
  * The path shards by string (SURVEY.md 8(e)): rank r of `world` scans the contiguous shard
  * pire_gpu_shard_bounds(n_global, world, r) -- boundaries on multiples of 32 strings, so bitmap words never straddle

@@ -175,6 +175,15 @@ private:
 // batch of streams is carried on in place round after round:
 //     Runner(gsc, BatchRunner::From(d_state)).Run(piece_k).Launch(nullptr, nullptr, d_state);          // round k
 //     Runner(gsc, BatchRunner::From(d_state)).Run(last).End().Launch(d_bits, d_masks, d_state);        // the last one
+// One frame of a LineStream (pire_gpu_line_frame): the lines of a text held in a device slot, as a line batch with the
+// offsets pire_gpu_split_lines makes, and where it lies in the whole text.  LineMatchEnds and HalfFinalCount take it as
+// a Batch; Runner(sc).Run(frame) scans it as the lines it holds (PIRE_GPU_RUN_LINES).
+struct LineFrame : Batch {
+    uint64_t Bytes = 0;          // bytes of Corpus
+    uint64_t FirstLine = 0;      // line 0 of the frame is line FirstLine of the text
+    uint64_t FirstByte = 0;      // Corpus[0] is byte FirstByte of the text
+};
+
 class BatchRunner {
 public:
     // n device words holding the StateIndex each string starts from (Runner(sc, st), run.h:391-392)
@@ -195,6 +204,7 @@ public:
     BatchRunner& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }      // run.h:375
     BatchRunner& End() { Flags |= PIRE_GPU_RUN_END; return *this; }          // run.h:376
     BatchRunner& Run(const Batch& b) { Input = b; Ran = true; return *this; } // run.h:372
+    BatchRunner& Run(const LineFrame& f) { Input = f; Flags |= PIRE_GPU_RUN_LINES; Ran = true; return *this; }
 
     // Launches the fused Begin/Run/End pass on `stream` (cudaStream_t as void*).
     void Launch(uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx, void* stream = nullptr) const
@@ -726,6 +736,55 @@ inline void MatchStarts(const Scanner& rsc, const LineMatchEnds& ends, uint64_t*
                                       ends.Ids, d_first, ends.Found, ends.Capacity, d_starts, d_open, ends.Stream),
           "pire_gpu_match_starts_lines");
 }
+
+// A text of any size from host memory as device frames of whole lines (pire_gpu_line_stream): Feed() takes the next
+// piece of the text, split anywhere, copies what fits into the next slot and returns how many bytes it took; the caller
+// feeds the rest again.  A frame is valid for work enqueued on `stream` before the next Feed() (pire_b200.h states
+// the exact rule); a frame may hold no lines.  One thread at a time.
+//     LineStream ls(0, 0, stream);
+//     LineStream::Frame f;
+//     for (const char* p = begin;;) {
+//         p += ls.Feed(p, end, /*last=*/true, f);
+//         Runner(gsc).Begin().Run(f).End().Launch(d_bits, nullptr, nullptr, stream);     // lines f.FirstLine + i
+//         if (p == end)
+//             break;
+//     }
+class LineStream {
+public:
+    typedef LineFrame Frame;
+
+    explicit LineStream(int device = 0, uint64_t slot_bytes = 0, void* stream = nullptr) : Handle(nullptr), Stream(stream)
+    {
+        Check(pire_gpu_line_stream_create(device, slot_bytes, &Handle), "pire_gpu_line_stream_create");
+    }
+    ~LineStream() { pire_gpu_line_stream_destroy(Handle); }
+    LineStream(const LineStream&) = delete;
+    LineStream& operator=(const LineStream&) = delete;
+
+    // The bytes [begin, end) with `last` = they end the text; returns the number taken.
+    size_t Feed(const char* begin, const char* end, bool last, Frame& frame)
+    {
+        uint64_t consumed = 0;
+        pire_gpu_line_frame f;
+        Check(pire_gpu_line_stream_feed(Handle, reinterpret_cast<const uint8_t*>(begin), (uint64_t) (end - begin), last ? 1 : 0,
+                                        Stream, &consumed, &f),
+              "pire_gpu_line_stream_feed");
+        frame.Corpus = f.d_text;
+        frame.Offsets = f.d_line_offsets;
+        frame.FixedLen = 0;
+        frame.Count = f.n_lines;
+        frame.Bytes = f.n_bytes;
+        frame.FirstLine = f.first_line;
+        frame.FirstByte = f.first_byte;
+        return (size_t) consumed;
+    }
+
+    pire_gpu_line_stream* Raw() const { return Handle; }
+
+private:
+    pire_gpu_line_stream* Handle;
+    void* Stream;
+};
 
 // AcceptedRegexps for scanners with more than 32 regexps: rows of AcceptWords(sc) words, bit r of row i set iff
 // regexp r is accepted by the state string i stopped in (d_state_idx from BatchRunner::Launch).

@@ -41,6 +41,7 @@ SYMBOLS = [
     "pire_gpu_match_ends_string", "pire_gpu_match_ends_batch_from",
     "pire_gpu_match_starts_string", "pire_gpu_match_starts_batch", "pire_gpu_run_pair_batch",
     "pire_gpu_match_ends_lines", "pire_gpu_match_starts_lines",
+    "pire_gpu_line_stream_create", "pire_gpu_line_stream_feed", "pire_gpu_line_stream_destroy",
 ]
 
 
@@ -49,6 +50,11 @@ class Info(C.Structure):
                 ("empty", C.c_uint32), ("hot_rows", C.c_uint32), ("variant", C.c_uint32), ("tuned", C.c_uint32),
                 ("table_bytes", C.c_uint64), ("shared_bytes", C.c_uint64), ("device", C.c_int32),
                 ("reserved", C.c_uint32)]
+
+
+class LineFrame(C.Structure):
+    _fields_ = [("d_text", C.c_void_p), ("d_line_offsets", C.c_void_p), ("n_lines", C.c_uint64), ("n_bytes", C.c_uint64),
+                ("first_line", C.c_uint64), ("first_byte", C.c_uint64)]
 
 
 class Synth(C.Structure):
@@ -91,6 +97,10 @@ def _load():
     lib.pire_gpu_match_ends_lines.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, C.c_uint64, vp, vp, vp, vp]
     lib.pire_gpu_match_starts_lines.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint32, C.c_uint64, vp, vp, vp, vp, vp, C.c_uint64,
                                                 vp, vp, vp]
+    lib.pire_gpu_line_stream_create.argtypes = [C.c_int, C.c_uint64, C.POINTER(vp)]
+    lib.pire_gpu_line_stream_feed.argtypes = [vp, vp, C.c_uint64, C.c_int, vp, C.POINTER(C.c_uint64), C.POINTER(LineFrame)]
+    lib.pire_gpu_line_stream_destroy.argtypes = [vp]
+    lib.pire_gpu_line_stream_destroy.restype = None
     lib.pire_gpu_length_order.argtypes = [vp, C.c_uint64, vp, C.c_int, vp]
     lib.pire_gpu_run_batch_ordered.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, vp]
     lib.pire_gpu_split_lines.argtypes = [vp, C.c_uint64, vp, C.c_uint64, C.POINTER(C.c_uint64), C.c_int, vp]

@@ -440,3 +440,209 @@ extern "C" int pire_gpu_run_batch_host(const pire_gpu_scanner* csc, const uint8_
     }
     return rc;
 }
+
+// ---- pire_gpu_line_stream: a text from host memory as device frames of whole lines --------------------------------
+//
+// Slot k % 3 receives the line carried over from slot (k - 1) % 3 (device to device) and then the new bytes (host to
+// device), all on the stream object's own stream.  The frame ends behind the last '\n' of the slot, found by a memrchr
+// over the new bytes on the host (the carry has no newline by construction), and pire_gpu_split_lines cuts it on the
+// device.  Before a slot is written, its stream waits for an event recorded on the caller's stream when the feed after
+// the slot's frame began: the caller's work on that frame.  Nothing waits for the work on the frame just returned.
+
+namespace pire_b200 {
+namespace {
+
+constexpr int kLineSlots = 3;
+constexpr uint64_t kLineSlotDefault = 256ull << 20;    // tools/line_stream_bench.py, DESIGN.md 4
+constexpr size_t kLinePad = 64;                // bytes behind a slot's text that vector loads may touch
+constexpr size_t kStagePiece = 8u << 20;       // pageable input: staged and sent in pieces, so the two overlap
+
+struct LineSlot {
+    uint8_t* d_text = nullptr;
+    size_t text_cap = 0;                       // bytes, kLinePad included
+    uint64_t* d_off = nullptr;
+    size_t off_cap = 0;                        // entries
+    uint64_t used = 0;                         // carry + new bytes in the slot
+    uint64_t framed = 0;                       // bytes of its frame; [framed, used) is carried to the next slot
+    cudaEvent_t released = nullptr;            // the caller's work on this slot's frame
+};
+
+} // namespace
+} // namespace pire_b200
+
+struct pire_gpu_line_stream {
+    int device = -1;
+    uint64_t slot_bytes = 0;
+    cudaStream_t copy = nullptr;
+    cudaEvent_t ready = nullptr;
+    pire_b200::LineSlot slot[pire_b200::kLineSlots];
+    uint8_t* h_stage = nullptr;
+    size_t stage_cap = 0;
+    pire_b200::CopyPool* pool = nullptr;
+    uint64_t frames = 0, first_line = 0, first_byte = 0;
+    bool finished = false;
+
+    ~pire_gpu_line_stream()
+    {
+        if (copy)
+            cudaStreamSynchronize(copy);
+        delete pool;
+        cudaFreeHost(h_stage);
+        for (pire_b200::LineSlot& s : slot) {
+            cudaFree(s.d_text);
+            cudaFree(s.d_off);
+            if (s.released)
+                cudaEventDestroy(s.released);
+        }
+        if (ready)
+            cudaEventDestroy(ready);
+        if (copy)
+            cudaStreamDestroy(copy);
+    }
+};
+
+namespace pire_b200 {
+namespace {
+
+int FeedLines(pire_gpu_line_stream* ls, const uint8_t* bytes, uint64_t n, bool last, cudaStream_t caller, uint64_t* consumed,
+              pire_gpu_line_frame* frame)
+{
+    LineSlot& s = ls->slot[ls->frames % kLineSlots];
+    LineSlot* prev = ls->frames ? &ls->slot[(ls->frames + kLineSlots - 1) % kLineSlots] : nullptr;
+    // the work the caller has enqueued on the previous frame so far is what its slot waits for three frames on
+    if (prev)
+        CUDA_TRY(cudaEventRecord(prev->released, caller));
+    const uint64_t carry = prev ? prev->used - prev->framed : 0;
+    // room for the new bytes: a slot, or twice the carry once the carry fills half of one (a line longer than a slot)
+    const uint64_t room = carry <= ls->slot_bytes / 2 ? ls->slot_bytes : 2 * carry;
+    const uint64_t take = std::min<uint64_t>(n, room - carry);
+    const uint64_t used = carry + take;
+
+    // the slot's last frame (three feeds ago) may still be read by the caller's kernels
+    CUDA_TRY(cudaStreamWaitEvent(ls->copy, s.released, 0));
+    const size_t off_want = (size_t) (ls->slot_bytes / 64 + 2);
+    if (s.text_cap < used + kLinePad || s.off_cap < off_want) {
+        CUDA_TRY(cudaEventSynchronize(s.released));          // buffers are freed below, not only overwritten
+        CUDA_TRY(GrowDevice(&s.d_text, &s.text_cap, (size_t) used + kLinePad));
+        CUDA_TRY(GrowDevice(&s.d_off, &s.off_cap, off_want));
+    }
+    if (carry)
+        CUDA_TRY(cudaMemcpyAsync(s.d_text, prev->d_text + prev->framed, carry, cudaMemcpyDeviceToDevice, ls->copy));
+    if (take) {
+        if (IsPinned(bytes)) {
+            CUDA_TRY(cudaMemcpyAsync(s.d_text + carry, bytes, take, cudaMemcpyHostToDevice, ls->copy));
+        } else {
+            if (!ls->pool) {
+                unsigned hw = std::thread::hardware_concurrency();
+                size_t threads = EnvSize("PIRE_B200_HOST_THREADS", std::min<size_t>(8, std::max<unsigned>(1, hw / 4)));
+                ls->pool = new CopyPool((unsigned) (threads > 1 ? threads - 1 : 0));
+            }
+            // the previous feed's copies from the staging buffer finished before it returned
+            CUDA_TRY(GrowPinned(&ls->h_stage, &ls->stage_cap, (size_t) take));
+            for (uint64_t at = 0; at < take; at += kStagePiece) {
+                const size_t len = (size_t) std::min<uint64_t>(kStagePiece, take - at);
+                ls->pool->Copy(ls->h_stage + at, bytes + at, len);
+                CUDA_TRY(cudaMemcpyAsync(s.d_text + carry + at, ls->h_stage + at, len, cudaMemcpyHostToDevice, ls->copy));
+            }
+        }
+    }
+    // the frame: through the last newline of the slot, or everything once the text has ended
+    const bool final = last && take == n;
+    const void* nl = take ? memrchr(bytes, '\n', (size_t) take) : nullptr;
+    const uint64_t framed = final ? used : nl ? carry + (uint64_t) (static_cast<const uint8_t*>(nl) - bytes) + 1 : 0;
+    uint64_t lines = 0;
+    if (framed) {
+        for (;;) {
+            int rc = pire_gpu_split_lines(s.d_text, framed, s.d_off, s.off_cap - 1, &lines, ls->device, ls->copy);
+            if (rc == PIRE_GPU_OK)
+                break;
+            if (rc != PIRE_GPU_EINVAL || lines < s.off_cap)
+                return rc;
+            CUDA_TRY(GrowDevice(&s.d_off, &s.off_cap, (size_t) (lines + lines / 4 + 2)));   // the slot was released above
+        }
+    } else {
+        CUDA_TRY(cudaMemsetAsync(s.d_off, 0, sizeof(uint64_t), ls->copy));
+    }
+    CUDA_TRY(cudaEventRecord(ls->ready, ls->copy));
+    CUDA_TRY(cudaStreamWaitEvent(caller, ls->ready, 0));
+    CUDA_TRY(cudaStreamSynchronize(ls->copy));                  // the caller's bytes are no longer referenced
+
+    s.used = used;
+    s.framed = framed;
+    *frame = pire_gpu_line_frame{s.d_text, s.d_off, lines, framed, ls->first_line, ls->first_byte};
+    *consumed = take;
+    ls->first_line += lines;
+    ls->first_byte += framed;
+    ++ls->frames;
+    ls->finished = final;
+    return PIRE_GPU_OK;
+}
+
+} // namespace
+} // namespace pire_b200
+
+extern "C" int pire_gpu_line_stream_create(int device, uint64_t slot_bytes, pire_gpu_line_stream** out)
+{
+    if (!out)
+        return Fail(PIRE_GPU_EINVAL, "out is null");
+    *out = nullptr;
+    if (device < 0)
+        return Fail(PIRE_GPU_ENODEVICE, "a line stream needs a CUDA device");
+    int count = 0;
+    cudaError_t ce = cudaGetDeviceCount(&count);
+    if (ce != cudaSuccess || device >= count) {
+        (void) cudaGetLastError();
+        return Fail(PIRE_GPU_ENODEVICE, ce != cudaSuccess ? std::string("no CUDA device: ") + cudaGetErrorString(ce)
+                                                          : std::string("CUDA device index out of range"));
+    }
+    CUDA_TRY(cudaSetDevice(device));
+    pire_gpu_line_stream* ls = new (std::nothrow) pire_gpu_line_stream;
+    if (!ls)
+        return Fail(PIRE_GPU_EINVAL, "out of memory");
+    ls->device = device;
+    ls->slot_bytes = slot_bytes ? slot_bytes : kLineSlotDefault;
+    cudaError_t err = cudaStreamCreateWithFlags(&ls->copy, cudaStreamNonBlocking);
+    if (err == cudaSuccess)
+        err = cudaEventCreateWithFlags(&ls->ready, cudaEventDisableTiming);
+    for (LineSlot& s : ls->slot)
+        if (err == cudaSuccess)
+            err = cudaEventCreateWithFlags(&s.released, cudaEventDisableTiming);
+    if (err != cudaSuccess) {
+        delete ls;
+        return FailCuda(err, "pire_gpu_line_stream_create");
+    }
+    *out = ls;
+    return PIRE_GPU_OK;
+}
+
+extern "C" int pire_gpu_line_stream_feed(pire_gpu_line_stream* ls, const uint8_t* bytes, uint64_t n, int last, void* stream,
+                                         uint64_t* consumed, pire_gpu_line_frame* frame)
+{
+    if (!ls || !consumed || !frame || (!bytes && n))
+        return Fail(PIRE_GPU_EINVAL, "null line stream, bytes, consumed or frame");
+    *consumed = 0;
+    if (ls->finished)
+        return Fail(PIRE_GPU_EINVAL, "feed after the last piece of the text");
+    CUDA_TRY(cudaSetDevice(ls->device));
+    int rc;
+    try {
+        rc = FeedLines(ls, bytes, n, last != 0, static_cast<cudaStream_t>(stream), consumed, frame);
+    } catch (const std::exception& e) {
+        rc = Fail(PIRE_GPU_EINVAL, std::string("pire_gpu_line_stream_feed: ") + e.what());
+    }
+    if (rc != PIRE_GPU_OK) {
+        *consumed = 0;
+        cudaStreamSynchronize(ls->copy);           // nothing in flight still points at the caller's bytes
+        (void) cudaGetLastError();
+    }
+    return rc;
+}
+
+extern "C" void pire_gpu_line_stream_destroy(pire_gpu_line_stream* ls)
+{
+    if (!ls)
+        return;
+    cudaSetDevice(ls->device);
+    cudaDeviceSynchronize();                       // the caller's work on the last frames reads the slots
+    delete ls;
+}

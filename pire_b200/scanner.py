@@ -107,6 +107,92 @@ class Batch:
         return int(o[self.n].item() - o[0].item()) - self.trim * self.n
 
 
+def _device_view(ptr, n, typestr, device):
+    """A CUDA tensor over n words of device memory the library owns (no copy)."""
+    class View:
+        __cuda_array_interface__ = {"shape": (int(n),), "typestr": typestr, "data": (int(ptr or 0), False), "version": 2,
+                                    "strides": None}
+    return _torch().as_tensor(View(), device=device)
+
+
+def _host_bytes(data):
+    """(address, length, owner) of the host bytes of ``bytes``, ``memoryview``, a numpy uint8 array or a CPU uint8
+    tensor (pinned or not); the owner keeps them alive."""
+    torch = _torch()
+    if isinstance(data, torch.Tensor):
+        if data.is_cuda or data.dtype != torch.uint8 or not data.is_contiguous():
+            raise ValueError("a tensor fed to a LineStream must be a contiguous uint8 CPU tensor")
+        return data.data_ptr(), data.numel(), data
+    arr = np.frombuffer(data, dtype=np.uint8) if isinstance(data, (bytes, bytearray, memoryview)) else data
+    if not isinstance(arr, np.ndarray) or arr.dtype != np.uint8 or arr.ndim != 1 or not arr.flags.c_contiguous:
+        raise ValueError("feed takes bytes, a memoryview, a contiguous 1-D numpy uint8 array or a uint8 CPU tensor")
+    return arr.ctypes.data, arr.size, arr
+
+
+class LineFrame(Batch):
+    """One frame of a ``LineStream``: a line batch (``trim`` = 1) of complete lines in a device slot of the stream, with
+    the offsets ``Batch.from_text`` would give for its bytes.  ``first_line`` and ``first_byte`` place it in the whole
+    text: line i of the frame is line first_line + i of the text, and frame position p is text position first_byte + p.
+    ``n_bytes`` is the length of the frame's text."""
+
+    def __init__(self, raw, device):
+        super().__init__(_device_view(raw.d_text, raw.n_bytes, "|u1", device),
+                         _device_view(raw.d_line_offsets, raw.n_lines + 1, "<i8", device), n=raw.n_lines)
+        self.trim = 1
+        self.n_bytes = int(raw.n_bytes)
+        self.first_line = int(raw.first_line)
+        self.first_byte = int(raw.first_byte)
+
+
+class LineStream:
+    """A text of any size from host memory, delivered to the device as frames of whole lines (pire_gpu_line_stream):
+    the text need not fit in HBM, and the copy of the next frame overlaps the work on the current one.
+
+        ls = LineStream(0)
+        for block in blocks:                       # pieces of the text, split anywhere
+            for frame in ls.feed(block, last=block is blocks[-1]):
+                hits = Runner(sc).Begin().Run(frame).End().Matches()
+
+    ``feed(data, last)`` is a generator: each frame is made when the caller asks for it, so a frame is never recycled
+    while the caller still works on it.  Work on a frame is enqueued on the current stream before the next frame is
+    asked for; the frame's tensors stay valid until that work has finished.  Frames without lines are not yielded.
+    ``data`` is ``bytes``, a ``memoryview``, a numpy uint8 array or a CPU uint8 tensor (pinned memory is DMA-ed
+    directly, pageable memory is staged by the library); it is no longer referenced when the generator is exhausted.
+    Exhaust one ``feed`` before the next; ``last=True`` ends the text (an unterminated last line becomes a line)."""
+
+    def __init__(self, device=0, slot_bytes=0):
+        h = C.c_void_p()
+        N.check(N.lib.pire_gpu_line_stream_create(int(device), int(slot_bytes), C.byref(h)), "pire_gpu_line_stream_create")
+        self._h = h
+        self.device = int(device)
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        lib = getattr(N, "lib", None)
+        if h and lib is not None:
+            lib.pire_gpu_line_stream_destroy(h)
+            self._h = None
+
+    def feed(self, data, last=False):
+        torch = _torch()
+        ptr, n, _owner = _host_bytes(data)
+        if n == 0 and not last:
+            return
+        dev = torch.device("cuda", self.device)
+        at = 0
+        while True:
+            consumed = C.c_uint64(0)
+            raw = N.LineFrame()
+            stream = torch.cuda.current_stream(dev).cuda_stream
+            N.check(N.lib.pire_gpu_line_stream_feed(self._h, ptr + at if n else None, n - at, 1 if last else 0, stream,
+                                                    C.byref(consumed), C.byref(raw)), "pire_gpu_line_stream_feed")
+            at += consumed.value
+            if raw.n_lines:
+                yield LineFrame(raw, dev)
+            if at == n:
+                return
+
+
 class Scanner:
     """A compiled multi-regexp scanner resident on one GPU (Pire::Scanner's role)."""
 

@@ -6,9 +6,16 @@
     python tools/pigrep.py [-i] [-u] -e PATTERN file [file ...]        # compile with the reference front end
                                                                        # (needs oracle/_ref; developer convenience)
     python tools/pigrep.py --half-final hf.pire --reverse rev.pire -o file [file ...]
+    zcat x.gz | python tools/pigrep.py --scanner patterns.pire            # no file, or "-": standard input
 
-Prints matching lines like pigrep (with a "file: " prefix when several files are given); -c prints counts only,
--n puts the line number (from 1) in front, -b the byte offset in the file of the line (or, with -o, of the match).
+Prints matching lines like pigrep (with a "file: " prefix when several files are given, "(stdin): " for "-"); -c
+prints counts only, -n puts the line number (from 1) in front, -b the byte offset in the file of the line (or, with -o,
+of the match).
+
+Every input, file or pipe, is read in blocks of --block-mb MiB (default 256) and streamed to the GPU through a
+LineStream (pire_gpu_line_stream): frames of whole lines, each scanned as it arrives, so an input of any size works and
+the GPU never holds more than three slots of it.  Line numbers and byte offsets are those of the whole input.  The
+bytes of a block are kept on the host until every frame that holds them has been printed.
 
 -o prints every match on a line of its own.  Where the matches end comes from a HalfFinalScanner image (--half-final:
 pire_gpu_match_ends_lines, every line its own run with BeginMark and EndMark), where they start from the same patterns
@@ -63,10 +70,10 @@ def main():
     ap.add_argument("-o", action="store_true", help="print every match on a line of its own")
     ap.add_argument("-n", action="store_true", help="prefix the line number")
     ap.add_argument("-b", action="store_true", help="prefix the byte offset of the line (with -o: of the match)")
-    ap.add_argument("files", nargs="+")
+    ap.add_argument("--block-mb", dest="block_mb", type=float, default=256.0,
+                    help="bytes read from an input at a time, in MiB (default 256)")
+    ap.add_argument("files", nargs="*", help="input files; none, or -, reads standard input")
     args = ap.parse_args()
-    import numpy as np
-    import torch
     import pire_b200 as P
     image = hf_image = rev_image = None
     if args.pattern:
@@ -84,36 +91,93 @@ def main():
         ap.error("-o needs --half-final FILE and --reverse FILE, or -e PATTERN")
     if not args.o and not image:
         ap.error("give --scanner FILE or -e PATTERN")
+    block = max(1, int(args.block_mb * (1 << 20)))
     sc = P.Scanner(image, 0) if image and not args.o else None
     hf = P.Scanner(hf_image, 0) if args.o else None
     rev = P.Scanner(rev_image, 0) if args.o else None
     out = sys.stdout.buffer
-    for name in args.files:
-        data = np.fromfile(name, dtype=np.uint8)
-        text = torch.from_numpy(data).to("cuda:0")
-        batch = P.Batch.from_text(text)
-        prefix = (name + ": ") if len(args.files) > 1 else ""
-        offs = batch.offsets.cpu().numpy()
-
-        def head(line, at):
-            return (prefix + ("%d:" % (line + 1) if args.n else "") + ("%d:" % at if args.b else "")).encode()
-
-        if args.o:
-            spans = line_spans(P, hf, rev, batch) if batch.n else {}
-            if args.c:
-                print("%s%d" % (prefix, len(spans)))
-                continue
-            for line in sorted(spans):
-                for s, e in spans[line]:
-                    out.write(head(line, s) + data[s:e].tobytes() + b"\n")
-            continue
-        hit = P.Runner(sc).Begin().Run(batch).End().Matches()
+    # samples/pigrep/pigrep.cpp: no file is stdin without a prefix; "-" is stdin, named "(stdin)" among several
+    names = args.files or [None]
+    for name in names:
+        prefix = ((name if name not in (None, "-") else "(stdin)") + ": ") if len(names) > 1 else ""
+        if name in (None, "-"):
+            count = grep_stream(P, args, sc, hf, rev, sys.stdin.buffer, block, prefix, out)
+        else:
+            with open(name, "rb") as f:
+                count = grep_stream(P, args, sc, hf, rev, f, block, prefix, out)
         if args.c:
-            print("%s%d" % (prefix, int(hit.sum())))
-            continue
-        for i in np.nonzero(hit)[0]:
-            out.write(head(int(i), int(offs[i])) + data[offs[i]: offs[i + 1] - 1].tobytes() + b"\n")
+            print("%s%d" % (prefix, count))
 
+
+def read_block(f, block):
+    """Up to `block` bytes of f (fewer only at the end of the input), read straight into a fresh numpy array."""
+    import numpy as np
+    buf = np.empty(block, dtype=np.uint8)
+    view, got = memoryview(buf), 0
+    while got < block:
+        k = f.readinto(view[got:])
+        if not k:
+            break
+        got += k
+    return buf[:got]
+
+
+class HeldText:
+    """The host bytes of the input from the first frame not yet printed on: the blocks read so far, by position."""
+
+    def __init__(self):
+        self.blocks = []            # (position of the block's first byte, numpy block)
+
+    def add(self, at, data):
+        self.blocks.append((at, data))
+
+    def bytes(self, lo, hi):
+        parts = [data[max(lo, at) - at: min(hi, at + len(data)) - at] for at, data in self.blocks
+                 if at < hi and at + len(data) > lo]
+        return b"".join(p.tobytes() for p in parts)
+
+    def drop_before(self, pos):
+        self.blocks = [(at, data) for at, data in self.blocks if at + len(data) > pos]
+
+
+def grep_stream(P, args, sc, hf, rev, f, block, prefix, out):
+    """Greps one input; prints the matches and returns the -c count."""
+    import numpy as np
+    ls = P.LineStream(0)
+    held = HeldText()
+    count, at = 0, 0
+
+    def head(line, pos):
+        return (prefix + ("%d:" % (line + 1) if args.n else "") + ("%d:" % pos if args.b else "")).encode()
+
+    last = False
+    while not last:
+        data = read_block(f, block)
+        last = len(data) < block
+        held.add(at, data)
+        at += len(data)
+        for frame in ls.feed(data, last=last):
+            line0, byte0 = frame.first_line, frame.first_byte
+            if args.o:
+                spans = line_spans(P, hf, rev, frame)
+                count += len(spans)
+                if args.c:
+                    continue
+                for line in sorted(spans):
+                    for s, e in spans[line]:
+                        out.write(head(line0 + line, byte0 + s) + held.bytes(byte0 + s, byte0 + e) + b"\n")
+            else:
+                hit = P.Runner(sc).Begin().Run(frame).End().Matches()
+                count += int(hit.sum())
+                if args.c:
+                    continue
+                offs = frame.offsets.cpu().numpy()
+                for i in np.nonzero(hit)[0]:
+                    lo, hi = byte0 + int(offs[i]), byte0 + int(offs[i + 1]) - 1
+                    out.write(head(line0 + int(i), lo) + held.bytes(lo, hi) + b"\n")
+            held.drop_before(byte0 + frame.n_bytes)
+    out.flush()
+    return count
 
 if __name__ == "__main__":
     main()

@@ -305,5 +305,19 @@ assert lfull.Found() == lpart.Found() == ltotal and (lpart.Ends() == lfull.Ends(
 key = lfull.Lines().astype(np.int64) * regs + lfull.Ids()
 assert (np.bincount(key, minlength=lb.n * regs).reshape(-1, regs) == lc.counts).all()
 print("ok match_ends_lines", flush=True)
+# a text streamed from host memory (pire_gpu_line_stream): pageable and pinned pieces, a line longer than the slot
+long_text = b"\n".join(s.replace(b"\n", b" ") for s in strings) + b"\n" + b"x" * 5000 + b"\nend"
+pinned = torch.empty(len(long_text), dtype=torch.uint8, pin_memory=True)
+pinned.copy_(torch.frombuffer(bytearray(long_text), dtype=torch.uint8))
+whole = P.Batch.from_text(torch.frombuffer(bytearray(long_text), dtype=torch.uint8).to("cuda:0"))
+want_bits = P.Runner(sc).Begin().Run(whole).End().Matches()
+ls = P.LineStream(0, 1024)
+got_bits = []
+half = len(long_text) // 2
+for k, piece in enumerate((np.frombuffer(long_text[:half], np.uint8), pinned[half:])):
+    for f in ls.feed(piece, last=k == 1):
+        got_bits += P.Runner(sc).Begin().Run(f).End().Matches().tolist()
+assert got_bits == want_bits.tolist()
+print("ok line_stream", flush=True)
 torch.cuda.synchronize()
 print("sanitize_run done, launches:", N.lib.pire_gpu_launch_count())
