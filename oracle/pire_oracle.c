@@ -218,11 +218,11 @@ void pire_oracle_run_batch(const pire_oracle_scanner* sc, const uint8_t* corpus,
         if (final_out)
             final_out[i] = (uint8_t) pire_oracle_final(sc, st);    /* run.h:380-381 */
         if (mask_out) {
-            uint64_t ids[64];
-            size_t k = pire_oracle_accepted(sc, st, ids, 64), j;
+            /* the whole accept list, however long (a list may name an id many times) */
+            const uint64_t* it = sc->empty ? 0 : sc->final_tab + sc->final_idx[pire_oracle_state_index(sc, st)];
             uint32_t m = 0;
-            for (j = 0; j < k && j < 64; ++j)
-                if (ids[j] < 32) m |= 1u << ids[j];
+            for (; it && *it != (uint64_t) -1; ++it)
+                if (*it < 32) m |= 1u << *it;
             mask_out[i] = m;
         }
         if (state_out)

@@ -400,6 +400,22 @@ void* pref_hf_load(const void* image, size_t size, char* err, size_t errlen)
 	}
 }
 
+// Scanner::Load (multi.h:575-599) of a stored Pire::Scanner image (Relocatable, ExitMasks<2>).  Only variants 0 and 1
+// answer for the handle: the NoMask variant cannot be made from a loaded image and stays empty.
+void* pref_load(const void* image, size_t size, char* err, size_t errlen)
+{
+	try {
+		std::istringstream in(std::string((const char*) image, size));
+		RefScanner* h = new RefScanner;
+		h->reloc.Load(&in);
+		h->MakeVariants();
+		return h;
+	} catch (std::exception& e) {
+		SetErr(err, errlen, e.what());
+		return nullptr;
+	}
+}
+
 void pref_hf_free(void* h) { delete (RefHalfFinal*) h; }
 int pref_hf_empty(void* h) { return ((RefHalfFinal*) h)->sc.Empty() ? 1 : 0; }
 uint64_t pref_hf_size(void* h) { return ((RefHalfFinal*) h)->sc.Size(); }

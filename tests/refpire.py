@@ -183,6 +183,12 @@ class Ref:
         lib.pref_hf_compile.argtypes = [C.c_char_p, C.c_char_p, C.c_int, C.c_char_p, C.c_size_t]
         lib.pref_hf_glue.restype = C.c_void_p
         lib.pref_hf_glue.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_char_p, C.c_size_t]
+        # pref_load came with the synthesized-image tests: a library built from an older oracle/ref_capi.cpp lacks it,
+        # and everything else still works with such a build
+        self.can_load = hasattr(lib, "pref_load")
+        if self.can_load:
+            lib.pref_load.restype = C.c_void_p
+            lib.pref_load.argtypes = [C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t]
         lib.pref_hf_load.restype = C.c_void_p
         lib.pref_hf_load.argtypes = [C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t]
         lib.pref_hf_free.argtypes = [C.c_void_p]
@@ -212,6 +218,16 @@ class Ref:
         if not h:
             raise ValueError(err.value.decode(errors="replace"))
         return RefHalfFinal(self.lib, h)
+
+    def load(self, image):
+        """Scanner::Load of a stored Pire::Scanner image; run, prefix and suffix take variant 0 or 1 on it."""
+        if not self.can_load:
+            raise RuntimeError("oracle/_ref/libpire_ref.so has no pref_load: rebuild it with oracle/build_ref.sh")
+        err = C.create_string_buffer(512)
+        h = self.lib.pref_load(bytes(image), len(image), err, len(err))
+        if not h:
+            raise ValueError(err.value.decode(errors="replace"))
+        return RefScanner(self.lib, h)
 
     def glue_half_final(self, a, b, max_size=0):
         err = C.create_string_buffer(512)
