@@ -203,7 +203,8 @@ int pire_gpu_run_batch_from(const pire_gpu_scanner* sc,
  * match bits.
  *   Batch   as pire_gpu_run_batch: CSR (d_offsets) or fixed length; no order.
  *   flags   PIRE_GPU_RUN_BEGIN and/or PIRE_GPU_RUN_END, stepped for both scanners; anything else (PIRE_GPU_RUN_LINES
- *           included) is PIRE_GPU_EINVAL, as are a NULL corpus with non-empty strings and n > 2^40.
+ *           included: the lines of a text have pire_gpu_run_pair_lines) is PIRE_GPU_EINVAL, as are a NULL corpus with
+ *           non-empty strings and n > 2^40.
  *   Start   d_start1 / d_start2: n device words each, or NULL for Initialize().  A start >= Size() yields match 0, mask
  *           0 and state 0xFFFFFFFF for its own scanner only.
  *   Chain   d_state_idx1 may be d_start1 and d_state_idx2 may be d_start2: both halves of a batch of streams are updated
@@ -478,6 +479,28 @@ int pire_gpu_split_lines(const uint8_t* d_text, uint64_t n_bytes, uint64_t* d_li
 int pire_gpu_run_lines(const pire_gpu_scanner* sc, const uint8_t* d_text, const uint64_t* d_line_offsets,
                        const uint32_t* d_order, uint64_t n_lines, uint32_t flags,
                        uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx, void* stream);
+
+/* Two scanners over the lines of a text.  Replaces, for every line of the text,
+ *     Pire::Runner(Pire::ScannerPair(sc1, sc2)) [.Begin()] .Run(line) [.End()]            scanners/pair.h
+ * for a pattern set split over two scanners, as pigrep with two scanners runs it.  Each scanner's three outputs are,
+ * bit for bit, what pire_gpu_run_lines(sc_k, d_text, d_line_offsets, NULL, n_lines, flags, ...) writes, the zeroed bits
+ * past n_lines in the last bitmap word included.  ScannerPair's Final() is the OR of the two match bits.
+ *   Lines   d_line_offsets are the offsets pire_gpu_split_lines made for d_text, as pire_gpu_run_lines requires.  Every
+ *           line starts from Initialize(); there is no order and no start state.
+ *   flags   PIRE_GPU_RUN_BEGIN and/or PIRE_GPU_RUN_END, stepped for both scanners; PIRE_GPU_RUN_LINES is implied and
+ *           accepted; anything else is PIRE_GPU_EINVAL, as are a NULL text or offsets with lines and n_lines >= 2^31.
+ *   Output  as pire_gpu_run_lines, once per scanner; each of the six may be NULL.  A buffer shared between the two
+ *           scanners' outputs is not supported.
+ *   Handles both on one device (PIRE_GPU_EINVAL otherwise); a host-only handle gets PIRE_GPU_ENODEVICE.  sc1 may be
+ *           sc2.  Each handle runs with its own hot set, tuned or not.
+ * When both start states are hot rows (practically always) the text is walked once: every byte is read from HBM once and
+ * walked through both automata.  Otherwise each scanner runs its own pire_gpu_run_lines launch, one after the other on
+ * the stream.  n_lines == 0 is a no-op.  Asynchronous on `stream`; re-entrant. */
+int pire_gpu_run_pair_lines(const pire_gpu_scanner* sc1, const pire_gpu_scanner* sc2,
+                            const uint8_t* d_text, const uint64_t* d_line_offsets, uint64_t n_lines, uint32_t flags,
+                            uint32_t* d_match_bits1, uint32_t* d_accept_masks1, uint32_t* d_state_idx1,
+                            uint32_t* d_match_bits2, uint32_t* d_accept_masks2, uint32_t* d_state_idx2,
+                            void* stream);
 
 /* Where the HalfFinalScanner matches end in every line of a text (grep -o, grep -n, grep -b): each line is its own run,
  * Runner(sc).Begin().Run(line).End() as samples/pigrep runs it, listed as pire_gpu_match_ends_batch_from lists a batch.

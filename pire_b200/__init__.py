@@ -3,7 +3,7 @@
 Only what the path needs lives here:
     csrc/         sm_90a CUDA kernels + the extern "C" boundary (include/pire_b200.h)
     _native.py    ctypes binding of that boundary (fails loudly if the .so is missing)
-    scanner.py    Python mirror of Pire's Scanner / Runner / Matches for batches (ScannerPair: two scanners at once),
+    scanner.py    Python mirror of Pire's Scanner / Runner / Matches for batches (ScannerPair: two scanners at once, over a batch or the lines of a text),
                   StringRunner, StringCounter and StringMatchEnds for one long string, BatchCounter and BatchMatchEnds for many streams,
                   LineMatchEnds for every line of a text, LineStream for a text streamed from host memory in frames of lines,
                   MatchStarts for the starts of either's matches

@@ -42,6 +42,7 @@ SYMBOLS = [
     "pire_gpu_match_starts_string", "pire_gpu_match_starts_batch", "pire_gpu_run_pair_batch",
     "pire_gpu_match_ends_lines", "pire_gpu_match_starts_lines",
     "pire_gpu_line_stream_create", "pire_gpu_line_stream_feed", "pire_gpu_line_stream_destroy",
+    "pire_gpu_run_pair_lines",
 ]
 
 
@@ -80,6 +81,7 @@ def _load():
     lib.pire_gpu_run_string.argtypes = [vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp]
     lib.pire_gpu_run_batch_from.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp]
     lib.pire_gpu_run_pair_batch.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.pire_gpu_run_pair_lines.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint32, vp, vp, vp, vp, vp, vp, vp]
     lib.pire_gpu_run_batch_host.argtypes = [vp, vp, C.c_uint64, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp]
     lib.pire_gpu_prefix_batch.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp]
     lib.pire_gpu_suffix_batch.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, C.c_int, vp, vp]

@@ -717,6 +717,48 @@ int pire_gpu_run_lines(const pire_gpu_scanner* sc, const uint8_t* d_text, const 
                   d_state_idx, stream);
 }
 
+int pire_gpu_run_pair_lines(const pire_gpu_scanner* sc1, const pire_gpu_scanner* sc2, const uint8_t* d_text,
+                            const uint64_t* d_line_offsets, uint64_t n_lines, uint32_t flags, uint32_t* d_match_bits1,
+                            uint32_t* d_accept_masks1, uint32_t* d_state_idx1, uint32_t* d_match_bits2, uint32_t* d_accept_masks2,
+                            uint32_t* d_state_idx2, void* stream)
+{
+    int rc = CheckRunnable(sc1);
+    if (rc == PIRE_GPU_OK)
+        rc = CheckRunnable(sc2);
+    if (rc != PIRE_GPU_OK)
+        return rc;
+    if (sc1->device != sc2->device)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_run_pair_lines needs two handles on one device");
+    if (flags & ~(PIRE_GPU_RUN_BEGIN | PIRE_GPU_RUN_END | PIRE_GPU_RUN_LINES))
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_run_pair_lines takes PIRE_GPU_RUN_BEGIN, PIRE_GPU_RUN_END and PIRE_GPU_RUN_LINES only");
+    if (n_lines == 0)
+        return PIRE_GPU_OK;
+    if (!d_text || !d_line_offsets)
+        return Fail(PIRE_GPU_EINVAL, "pire_gpu_run_pair_lines needs the text and its line offsets");
+    if (n_lines >= (1ull << 31))
+        return Fail(PIRE_GPU_EINVAL, "too many lines");
+    CUDA_TRY(cudaSetDevice(sc1->device));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    ScanArgs a[2];
+    int variant[2];
+    const pire_gpu_scanner* sc[2] = {sc1, sc2};
+    uint32_t* bits[2] = {d_match_bits1, d_match_bits2};
+    uint32_t* masks[2] = {d_accept_masks1, d_accept_masks2};
+    uint32_t* states[2] = {d_state_idx1, d_state_idx2};
+    for (int k = 0; k < 2; ++k) {
+        FillArgs(sc[k], &a[k], d_text, d_line_offsets, 0, n_lines, flags | PIRE_GPU_RUN_LINES);
+        a[k].match_bits = bits[k];
+        a[k].accept_masks = masks[k];
+        a[k].state_idx = states[k];
+        variant[k] = (int) BatchVariant(sc[k], false, n_lines);
+        // match bits are OR-ed into a zeroed bitmap, as pire_gpu_run_lines does
+        if (bits[k])
+            CUDA_TRY(cudaMemsetAsync(bits[k], 0, (size_t) ((n_lines + 31) / 32) * 4, st));
+    }
+    CUDA_TRY(LaunchPairLines(a[0], a[1], variant[0], variant[1], sc1->device, st));
+    return PIRE_GPU_OK;
+}
+
 static int RunCsr(const pire_gpu_scanner* sc, const uint8_t* d_corpus, const uint64_t* d_offsets, const uint32_t* d_order,
                   uint64_t n, uint32_t flags, uint32_t* d_match_bits, uint32_t* d_accept_masks, uint32_t* d_state_idx,
                   void* stream, const uint32_t* d_start)

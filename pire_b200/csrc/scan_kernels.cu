@@ -2371,6 +2371,216 @@ __global__ void __launch_bounds__(kBlock, kTextBlocksPerSM) ScanTextKernel(const
     }
 }
 
+// ---------------------------------------------------------------- two scanners over the lines of a text, in stream
+//
+// pire_gpu_run_pair_lines: ScanTextKernel's walk with two chains, one per scanner.  The text is cut into the same
+// segments and a lane owns the same lines; every 32-byte block is loaded once and its newlines found once, and each
+// byte advances both chains, in turn, so that chain b's table read fills the latency of chain a's.  Each chain has its
+// own copy of its hot rows ('\n' leading to its own start state), class map, exit filter ('\n' let through) and copy
+// of the hot states' reports.  The states in front of the bytes are packed per chain, so each newline reports both
+// scanners' state for the line.
+// The line cursor (TextLane) is shared: it moves once per newline, for both chains together.  When either chain
+// leaves its hot rows in a block, the block is replayed byte by byte for BOTH chains from the states they had in front
+// of it (TextSlow2); otherwise the newline loop reports both chains from the packed states.  Exactly one of the two
+// runs for a block, and each reports every line that ends in the block once per chain, so no line is reported twice
+// and the cursor moves once per newline.  Replaying a chain that stayed in its hot rows is exact: the complete table
+// gives the states the hot rows gave, and TextSlow2 restarts at '\n' as the hot rows do.
+// Shared memory: chain a's tables at 0, chain b's at kPairSecond (room for any hot set), then the two copies of the hot
+// reports (2 x 2 KiB) and the packed states (32 bytes per thread and chain): 188 416 bytes at most at 512 threads, so
+// neither hot set is ever cut and one CTA runs per SM.  512 threads: on an H100 the kernel took 9.3-9.5 ms for two
+// scanners over 4 GiB of lines, against 11.4-11.5 ms at 768 and 13.4-13.8 ms at 1 024 (DESIGN.md 4); one CTA of 512
+// threads leaves it 128 registers, and it uses 72.
+constexpr int kPairTextBlock = 512;
+
+// Four steps of both chains; qa / qb collect the states in front of the bytes as TextWord does.
+__device__ __forceinline__ void TextWord2(const Tables& ta, uint32_t& ga, uint32_t& qa, const Tables& tb, uint32_t& gb, uint32_t& qb,
+                                          uint32_t w)
+{
+#pragma unroll
+    for (uint32_t i = 0; i < 4; ++i) {
+        asm("mad.lo.u32 %0, %0, 256, %1;" : "+r"(qa) : "r"(ga));
+        FastStep<true>(ta, ga, w, 0x5540u + i);
+        asm("mad.lo.u32 %0, %0, 256, %1;" : "+r"(qb) : "r"(gb));
+        FastStep<true>(tb, gb, w, 0x5540u + i);
+    }
+}
+
+// TextSlow for both chains from the complete states fa / fb: one cursor step per newline.
+__device__ __forceinline__ void TextSlow2(const PairArgs& p, const Tables& ta, const Tables& tb, const DeviceFin* fin_a,
+                                          const DeviceFin* fin_b, uint32_t outs_a, uint32_t outs_b, TextLane& c, LaneState& sa,
+                                          LaneState& sb, uint32_t fa, uint32_t fb, int64_t cpos, uint32_t from, uint32_t to,
+                                          uint64_t seg_hi, uint64_t total)
+{
+    const ScanArgs& a = p.s[0];
+    const ScanArgs& b = p.s[1];
+    for (uint32_t j = from; j < to; ++j) {
+        const uint64_t at = (uint64_t) (cpos + (int64_t) j);
+        const uint32_t byte = at < total ? a.corpus[at] : (uint32_t) '\n';
+        if (byte == '\n') {
+            TextReport(a, outs_a, c.line, fa < ta.H ? fin_a[fa] : a.fin[fa]);
+            TextReport(b, outs_b, c.line, fb < tb.H ? fin_b[fb] : b.fin[fb]);
+            ++c.line;
+            fa = a.start;
+            fb = b.start;
+            if (c.line >= a.n || at + 1 >= seg_hi) {
+                c.active = false;
+                break;
+            }
+            continue;
+        }
+        fa = SlowStep(ta, fa, byte);
+        fb = SlowStep(tb, fb, byte);
+    }
+    SetFull(ta, sa, fa);
+    SetFull(tb, sb, fb);
+}
+
+// TextBlock for both chains.  `packs` as in TextBlock; chain b's packed states lie 1 KiB behind chain a's.
+__device__ __forceinline__ void TextBlock2(const PairArgs& p, const Tables& ta, const Tables& tb, const DeviceFin* fin_a,
+                                           const DeviceFin* fin_b, uint32_t outs_a, uint32_t outs_b, TextLane& c, LaneState& sa,
+                                           LaneState& sb, uint4 v0, uint4 v1, uint32_t packs, int64_t cpos, uint64_t seg_hi,
+                                           uint64_t total)
+{
+    const uint32_t before_a = sa.g, before_b = sb.g;
+    uint32_t ga = before_a, gb = before_b;
+    uint4 qa0 = make_uint4(0, 0, 0, 0), qa1 = qa0, qb0 = qa0, qb1 = qa0;
+    TextWord2(ta, ga, qa0.x, tb, gb, qb0.x, v0.x);
+    TextWord2(ta, ga, qa0.y, tb, gb, qb0.y, v0.y);
+    TextWord2(ta, ga, qa0.z, tb, gb, qb0.z, v0.z);
+    TextWord2(ta, ga, qa0.w, tb, gb, qb0.w, v0.w);
+    TextWord2(ta, ga, qa1.x, tb, gb, qb1.x, v1.x);
+    TextWord2(ta, ga, qa1.y, tb, gb, qb1.y, v1.y);
+    TextWord2(ta, ga, qa1.z, tb, gb, qb1.z, v1.z);
+    TextWord2(ta, ga, qa1.w, tb, gb, qb1.w, v1.w);
+    const int32_t left = c.left;
+    c.left = left - 32 > -(1 << 30) ? left - 32 : -(1 << 30);
+    if (!c.active)
+        return;
+    if (ga == ta.H || gb == tb.H) {
+        // either chain was, or fell, outside its hot rows: the block again for both, the cursor moved by the replay alone
+        TextSlow2(p, ta, tb, fin_a, fin_b, outs_a, outs_b, c, sa, sb, before_a == ta.H ? sa.cold : before_a,
+                  before_b == tb.H ? sb.cold : before_b, cpos, 0, 32, seg_hi, total);
+        return;
+    }
+    sa.g = ga;
+    sb.g = gb;
+    uint32_t ends = NewlineNibble(v0.x) | (NewlineNibble(v0.y) << 4) | (NewlineNibble(v0.z) << 8) | (NewlineNibble(v0.w) << 12) |
+                    (NewlineNibble(v1.x) << 16) | (NewlineNibble(v1.y) << 20) | (NewlineNibble(v1.z) << 24) | (NewlineNibble(v1.w) << 28);
+    if (ends == 0)
+        return;
+    asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(packs), "r"(qa0.x), "r"(qa0.y), "r"(qa0.z), "r"(qa0.w) : "memory");
+    asm volatile("st.shared.v4.u32 [%0+512], {%1,%2,%3,%4};" ::"r"(packs), "r"(qa1.x), "r"(qa1.y), "r"(qa1.z), "r"(qa1.w) : "memory");
+    asm volatile("st.shared.v4.u32 [%0+1024], {%1,%2,%3,%4};" ::"r"(packs), "r"(qb0.x), "r"(qb0.y), "r"(qb0.z), "r"(qb0.w) : "memory");
+    asm volatile("st.shared.v4.u32 [%0+1536], {%1,%2,%3,%4};" ::"r"(packs), "r"(qb1.x), "r"(qb1.y), "r"(qb1.z), "r"(qb1.w) : "memory");
+    const uint32_t n_lines = (uint32_t) p.s[0].n;
+    do {
+        const uint32_t k = (uint32_t) __ffs((int) ends) - 1u;
+        ends &= ends - 1u;
+        const uint32_t at = packs + ((k & 16u) << 5) + ((k & 15u) ^ 3u);
+        uint32_t st_a, st_b;
+        asm volatile("ld.shared.u8 %0, [%1];" : "=r"(st_a) : "r"(at) : "memory");
+        asm volatile("ld.shared.u8 %0, [%1+1024];" : "=r"(st_b) : "r"(at) : "memory");
+        TextReport(p.s[0], outs_a, c.line, fin_a[st_a]);
+        TextReport(p.s[1], outs_b, c.line, fin_b[st_b]);
+        ++c.line;
+        if (c.line >= n_lines || (int32_t) k + 1 >= left) {
+            c.active = false;
+            break;
+        }
+    } while (ends);
+}
+
+__device__ __forceinline__ void PairTextTables(const ScanArgs& a, const SharedView& sv, Tables& t)
+{
+    t.hot = sv.hot;
+    t.base = SmemAddr(sv.hot);
+    t.cls = sv.cls;
+    t.full = a.full;
+    t.H = a.hot;
+    t.letters = a.letters;
+    t.wide = a.wide;
+    t.m0 = a.exit_bitmap0 | (1u << ('\n' & 31));
+}
+
+__global__ void __launch_bounds__(kPairTextBlock, 1) ScanTextPairKernel(const __grid_constant__ PairArgs p)
+{
+    const ScanArgs& a = p.s[0];
+    const ScanArgs& b = p.s[1];
+    uint8_t* const smem = pire_b200_smem;
+    const SharedView sva = CarveShared(smem, a.hot);
+    const SharedView svb = CarveShared(smem + kPairSecond, b.hot);
+    StageTables(a, sva, a.hot8, a.hot);
+    StageTables(b, svb, b.hot8, b.hot);
+    DeviceFin* const fin_a = reinterpret_cast<DeviceFin*>(svb.stage);
+    DeviceFin* const fin_b = fin_a + 256;
+    for (uint32_t g = threadIdx.x; g < a.hot; g += blockDim.x) {
+        sva.hot[g * kHotStride + '\n'] = (uint8_t) a.start;
+        fin_a[g] = a.fin[g];
+    }
+    for (uint32_t g = threadIdx.x; g < b.hot; g += blockDim.x) {
+        svb.hot[g * kHotStride + '\n'] = (uint8_t) b.start;
+        fin_b[g] = b.fin[g];
+    }
+    __syncthreads();
+
+    Tables ta, tb;
+    PairTextTables(a, sva, ta);
+    PairTextTables(b, svb, tb);
+
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t outs_a = TextOutputs(a);
+    const uint32_t outs_b = TextOutputs(b);
+    const uint32_t packs = SmemAddr(svb.stage) + 2 * (uint32_t) kTextFinBytes + (threadIdx.x >> 5) * 2048u + lane * 16u;
+    const uint64_t total = a.offsets[a.n] - 1;
+    const uintptr_t buf_lo = reinterpret_cast<uintptr_t>(a.corpus);
+    const uintptr_t buf_hi = buf_lo + total;
+    const uint32_t mis0 = (uint32_t) (buf_lo & 31);
+    const uint64_t warps = (uint64_t) gridDim.x * (kPairTextBlock / 32);
+    const TextSegments segs = TextSegmentsOf(total, mis0, warps);
+
+    for (uint64_t unit = (uint64_t) blockIdx.x * (kPairTextBlock / 32) + (threadIdx.x >> 5); unit < segs.units; unit += warps) {
+        const uint64_t sidx = unit * 32 + lane;
+        const uint64_t seg_hi = (sidx + 1) * segs.seg - mis0;
+        TextLane c;
+        c.line = 0;
+        c.left = 0;
+        c.active = false;
+        LaneState sa, sb;
+        sa.g = a.start;
+        sa.cold = 0;
+        sb.g = b.start;
+        sb.cold = 0;
+        const uint8_t* q = a.corpus;
+        int64_t pos = 0;
+        uint64_t line = 0, pos0 = 0;
+        if (sidx < segs.segments && TextFirstLine(a, sidx, segs.seg, mis0, seg_hi, line, pos0)) {
+            c.line = (uint32_t) line;
+            c.active = true;
+            pos = (int64_t) ((pos0 + mis0) & ~31ull) - (int64_t) mis0;      // the 32-byte block the line starts in
+            const uint32_t skip = (uint32_t) ((int64_t) pos0 - pos);
+            if (skip) {
+                TextSlow2(p, ta, tb, fin_a, fin_b, outs_a, outs_b, c, sa, sb, a.start, b.start, pos, skip, 32, seg_hi, total);
+                pos += 32;
+            }
+            q = a.corpus + pos;
+            c.left = (int32_t) ((int64_t) seg_hi - pos);
+        }
+        uint4 v0 = make_uint4(0, 0, 0, 0), v1 = v0;
+        if (c.active)
+            LoadBlock32(q, buf_lo, buf_hi, v0, v1);
+        while (__any_sync(0xffffffffu, c.active)) {
+            uint4 n0 = make_uint4(0, 0, 0, 0), n1 = n0;
+            if (c.active)
+                LoadBlock32(q + 32, buf_lo, buf_hi, n0, n1);
+            TextBlock2(p, ta, tb, fin_a, fin_b, outs_a, outs_b, c, sa, sb, v0, v1, packs, pos, seg_hi, total);
+            v0 = n0;
+            v1 = n1;
+            q += 32;
+            pos += 32;
+        }
+    }
+}
+
 // ---------------------------------------------------------------- PRIV variant
 //
 // The plain walk is bound by shared-memory wavefronts once lanes sit in different
@@ -4978,6 +5188,41 @@ cudaError_t LaunchLines(const ScanArgs& a, int variant, int device, cudaStream_t
     }
     void* args[] = {&tuned};
     err = cudaLaunchKernel(fn, dim3(grid), dim3(kBlock), args, shared, stream);
+    if (err == cudaSuccess)
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+    return err;
+}
+
+// Two scanners over the lines of a text (pire_gpu_run_pair_lines).  In stream for both (ScanTextPairKernel) when both
+// start states are hot rows; otherwise each scanner's own LaunchLines, one after the other on the stream.
+cudaError_t LaunchPairLines(const ScanArgs& a, const ScanArgs& b, int variant_a, int variant_b, int device, cudaStream_t stream)
+{
+    if (a.n == 0)
+        return cudaSuccess;
+    if (a.start >= a.hot || b.start >= b.hot) {
+        cudaError_t err = LaunchLines(a, variant_a, device, stream);
+        return err == cudaSuccess ? LaunchLines(b, variant_b, device, stream) : err;
+    }
+    const void* fn = reinterpret_cast<const void*>(&ScanTextPairKernel);
+    const size_t shared = kPairSecond + ScanSharedBytes(b.hot, 0) + 2 * kTextFinBytes + (size_t) kPairTextBlock * 64;
+    int optin = 0, sms = 0, per_sm = 0;
+    cudaError_t err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+    if (err == cudaSuccess)
+        err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err == cudaSuccess)
+        err = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+    if (err == cudaSuccess)
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fn, kPairTextBlock, shared);
+    if (err != cudaSuccess)
+        return err;
+    if (per_sm < 1)
+        return cudaErrorLaunchOutOfResources;
+    PairArgs p;
+    p.s[0] = a;
+    p.s[1] = b;
+    void* args[] = {&p};
+    // the persistent grid is launched whole, as in LaunchLines
+    err = cudaLaunchKernel(fn, dim3(sms * per_sm), dim3(kPairTextBlock), args, shared, stream);
     if (err == cudaSuccess)
         g_launches.fetch_add(1, std::memory_order_relaxed);
     return err;

@@ -146,6 +146,10 @@ cudaError_t LaunchScan(const ScanArgs& a, int variant, bool uniform, const Launc
 cudaError_t LaunchPair(const ScanArgs& a, const ScanArgs& b, int device, cudaStream_t stream);
 // CSR batches of short strings (lines of text): lanes pull strings dynamically; a.match_bits must be zeroed
 cudaError_t LaunchLines(const ScanArgs& a, int variant, int device, cudaStream_t stream);
+// Two scanners over the lines of a text (ScanTextPairKernel, pire_gpu_run_pair_lines): a and b are what LaunchLines would
+// take for each scanner alone (the same text, offsets and n; both bitmaps zeroed), variant_a / variant_b its variant.
+// Fused when both start states are hot rows; otherwise the two LaunchLines calls, one after the other on the stream.
+cudaError_t LaunchPairLines(const ScanArgs& a, const ScanArgs& b, int variant_a, int variant_b, int device, cudaStream_t stream);
 // length-ordered CSR batches: the leading long strings, one per warp; sets *a.split_count, which the generic launch honours
 cudaError_t LaunchSplit(const ScanArgs& a, int variant, int device, cudaStream_t stream);
 // one string (a.corpus, a.fixed_len bytes) over the whole grid, cooperatively launched; a.with_begin / a.begin_class

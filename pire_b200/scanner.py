@@ -426,7 +426,8 @@ class RunHelper:
 
 class ScannerPair:
     """Pire::ScannerPair<S1, S2> (scanners/pair.h): two scanners stepped over the same bytes in lock-step.  ``Runner(pair)``
-    scans a batch once for both (pire_gpu_run_pair_batch); the two may be the same Scanner."""
+    scans a batch once for both (pire_gpu_run_pair_batch), ``Runner(pair).RunLines(lines)`` the lines of a text
+    (pire_gpu_run_pair_lines); the two may be the same Scanner."""
 
     def __init__(self, first, second):
         self.First, self.Second = first, second
@@ -448,6 +449,19 @@ class ScannerPair:
                                               *[ptr(t) for t in tuple(outs1) + tuple(outs2)], stream),
                 "pire_gpu_run_pair_batch")
 
+    def run_pair_lines(self, lines, flags, outs1, outs2, stream=None):
+        """Thin wrapper of pire_gpu_run_pair_lines: ``lines`` is a line batch (``Batch.from_text`` or a ``LineFrame``),
+        ``outs1`` / ``outs2`` are (match_bits, accept_masks, state_idx) tensors, any of them None."""
+        torch = _torch()
+        if stream is None:
+            stream = torch.cuda.current_stream(lines.device).cuda_stream
+        if not getattr(lines, "trim", 0) or getattr(lines, "order", None) is not None:
+            raise ValueError("run_pair_lines takes the lines of a text (Batch.from_text or a LineFrame), without an order")
+        ptr = lambda t: None if t is None else t.data_ptr()
+        N.check(N.lib.pire_gpu_run_pair_lines(self.First._h, self.Second._h, lines.corpus.data_ptr(), ptr(lines.offsets),
+                                              lines.n, flags, *[ptr(t) for t in tuple(outs1) + tuple(outs2)], stream),
+                "pire_gpu_run_pair_lines")
+
 
 class _PairHalf(RunHelper):
     """One scanner's view of a PairRunHelper: RunHelper's results, filled in by the pair's one launch."""
@@ -466,7 +480,11 @@ class PairRunHelper:
     ``Second()`` are each scanner's RunHelper results.
 
     ``states`` = (states1, states2), either None, starts each scanner's strings from its own states (Runner(sc, st) per
-    string); ``Runner(pair, (r.First().StateTensor(), r.Second().StateTensor()))`` carries a batch of streams on."""
+    string); ``Runner(pair, (r.First().StateTensor(), r.Second().StateTensor()))`` carries a batch of streams on.
+
+    The lines of a text go through ``RunLines(lines)`` (a ``Batch.from_text`` batch or a ``LineFrame``;
+    pire_gpu_run_pair_lines): every line is its own run for both scanners, and the text is walked once.  ``Run()`` takes
+    plain batches only and refuses a line batch with ValueError."""
 
     def __init__(self, pair, states=None):
         self.Pair = pair
@@ -474,7 +492,7 @@ class PairRunHelper:
         if len(self._starts) != 2:
             raise ValueError("states is a pair (states1, states2)")
         self._halves = (_PairHalf(self, pair.First), _PairHalf(self, pair.Second))
-        self._begin = self._end = self._ran = False
+        self._begin = self._end = self._ran = self._lines = False
 
     def Begin(self):
         if self._halves[0]._batch is not None:
@@ -487,6 +505,16 @@ class PairRunHelper:
             raise ValueError("one Run() per RunHelper on the batch path")
         for h in self._halves:
             h._batch = batch
+        return self
+
+    def RunLines(self, lines):
+        """The lines of a text (``Batch.from_text`` or a ``LineFrame``), each its own run for both scanners."""
+        if not getattr(lines, "trim", 0):
+            raise ValueError("RunLines takes the lines of a text (Batch.from_text or a LineFrame)")
+        if self._starts != (None, None):
+            raise ValueError("lines start from Initialize(): no start states")
+        self.Run(lines)
+        self._lines = True
         return self
 
     def End(self):
@@ -507,7 +535,10 @@ class PairRunHelper:
             h._states = torch.empty(b.n, dtype=torch.int32, device=b.device)
             outs.append((h._bits, h._masks, h._states))
         flags = (N.RUN_BEGIN if self._begin else 0) | (N.RUN_END if self._end else 0)
-        self.Pair.run_pair_batch(b, flags, outs[0], outs[1], self._starts)
+        if self._lines:
+            self.Pair.run_pair_lines(b, flags, outs[0], outs[1])
+        else:
+            self.Pair.run_pair_batch(b, flags, outs[0], outs[1], self._starts)
         self._ran = True
 
     def First(self):

@@ -3,6 +3,7 @@
 (std::getline + Runner(sc).Begin().Run(line).End()) moved to the device.
 
     python tools/pigrep.py --scanner patterns.pire file [file ...]     # precompiled Scanner::Save() image
+    python tools/pigrep.py --scanner a.pire --scanner b.pire file ...  # a pattern set glued into two scanners
     python tools/pigrep.py [-i] [-u] -e PATTERN file [file ...]        # compile with the reference front end
                                                                        # (needs oracle/_ref; developer convenience)
     python tools/pigrep.py --half-final hf.pire --reverse rev.pire -o file [file ...]
@@ -11,6 +12,10 @@
 Prints matching lines like pigrep (with a "file: " prefix when several files are given, "(stdin): " for "-"); -c
 prints counts only, -n puts the line number (from 1) in front, -b the byte offset in the file of the line (or, with -o,
 of the match).
+
+--scanner may be given twice, for a pattern set that Scanner::Glue could not put into one scanner: a line is printed
+when either scanner accepts it (ScannerPair's Final()), and each frame is scanned once for both
+(pire_gpu_run_pair_lines).  -c, -n and -b keep their meaning.
 
 Every input, file or pipe, is read in blocks of --block-mb MiB (default 256) and streamed to the GPU through a
 LineStream (pire_gpu_line_stream): frames of whole lines, each scanned as it arrives, so an input of any size works and
@@ -23,8 +28,8 @@ compiled with Fsm::Reverse() (--reverse: pire_gpu_match_starts_lines, the leftmo
 (start, end) pairs of a line, non-empty spans are taken leftmost-longest and without overlap: sorted by start
 ascending, then end descending, a span is taken when it starts at or after the end of the span taken before it.  That
 is close to what grep -o prints, but it is this selection over Pire's spans, not GNU grep's matcher, and the two can
-differ.  With -o, -c counts the lines that have at least one span.  With -e all three scanners are compiled from the
-pattern.
+differ.  With -o, -c counts the lines that have at least one span, and --scanner is not used.  With -e all three
+scanners are compiled from the pattern.
 """
 import argparse
 import os
@@ -60,7 +65,8 @@ def line_spans(P, hf, rev, batch):
 
 def main():
     ap = argparse.ArgumentParser(add_help=True)
-    ap.add_argument("--scanner")
+    ap.add_argument("--scanner", action="append", default=[],
+                    help="Scanner::Save() image; give it twice for a pattern set split over two scanners")
     ap.add_argument("--half-final", dest="half_final", help="HalfFinalScanner image of the patterns (-o)")
     ap.add_argument("--reverse", help="Scanner image of the patterns built with Fsm::Reverse() (-o)")
     ap.add_argument("-e", dest="pattern")
@@ -75,24 +81,27 @@ def main():
     ap.add_argument("files", nargs="*", help="input files; none, or -, reads standard input")
     args = ap.parse_args()
     import pire_b200 as P
-    image = hf_image = rev_image = None
+    images, hf_image, rev_image = [], None, None
     if args.pattern:
         sys.path.insert(0, os.path.join(ROOT, "tests"))
         from refpire import Ref           # the reference's own Lexer/Fsm/Compile, unchanged host code
         ref, opts = Ref(), ("i" if args.i else "") + ("u" if args.u else "")
-        image = ref.compile(args.pattern.encode(), opts).save()
+        images = [ref.compile(args.pattern.encode(), opts).save()]
         hf_image = ref.compile_half_final(args.pattern.encode(), opts).save()
         rev_image = ref.compile(args.pattern.encode(), opts + "nr").save()
     else:
-        image = open(args.scanner, "rb").read() if args.scanner else None
+        images = [open(name, "rb").read() for name in args.scanner]
         hf_image = open(args.half_final, "rb").read() if args.half_final else None
         rev_image = open(args.reverse, "rb").read() if args.reverse else None
     if args.o and not (hf_image and rev_image):
         ap.error("-o needs --half-final FILE and --reverse FILE, or -e PATTERN")
-    if not args.o and not image:
+    if not args.o and not images:
         ap.error("give --scanner FILE or -e PATTERN")
+    if len(images) > 2:
+        ap.error("--scanner may be given at most twice")
     block = max(1, int(args.block_mb * (1 << 20)))
-    sc = P.Scanner(image, 0) if image and not args.o else None
+    scanners = [P.Scanner(image, 0) for image in images] if not args.o else []
+    sc = scanners[0] if len(scanners) == 1 else P.ScannerPair(*scanners) if scanners else None
     hf = P.Scanner(hf_image, 0) if args.o else None
     rev = P.Scanner(rev_image, 0) if args.o else None
     out = sys.stdout.buffer
@@ -141,7 +150,7 @@ class HeldText:
 
 
 def grep_stream(P, args, sc, hf, rev, f, block, prefix, out):
-    """Greps one input; prints the matches and returns the -c count."""
+    """Greps one input; prints the matches and returns the -c count.  `sc` is a Scanner or a ScannerPair."""
     import numpy as np
     ls = P.LineStream(0)
     held = HeldText()
@@ -167,7 +176,10 @@ def grep_stream(P, args, sc, hf, rev, f, block, prefix, out):
                     for s, e in spans[line]:
                         out.write(head(line0 + line, byte0 + s) + held.bytes(byte0 + s, byte0 + e) + b"\n")
             else:
-                hit = P.Runner(sc).Begin().Run(frame).End().Matches()
+                if isinstance(sc, P.ScannerPair):
+                    hit = P.Runner(sc).Begin().RunLines(frame).End().Matches()
+                else:
+                    hit = P.Runner(sc).Begin().Run(frame).End().Matches()
                 count += int(hit.sum())
                 if args.c:
                     continue

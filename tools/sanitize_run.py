@@ -319,5 +319,13 @@ for k, piece in enumerate((np.frombuffer(long_text[:half], np.uint8), pinned[hal
         got_bits += P.Runner(sc).Begin().Run(f).End().Matches().tolist()
 assert got_bits == want_bits.tolist()
 print("ok line_stream", flush=True)
+# two scanners over the lines of that text in one walk (pire_gpu_run_pair_lines), against the two single calls
+other = P.Scanner(W.load_image("headline"), 0)
+both = P.Runner(P.ScannerPair(sc, other)).Begin().RunLines(whole).End()
+for half_, one in ((both.First(), sc), (both.Second(), other)):
+    ref = P.Runner(one).Begin().Run(whole).End()
+    assert (half_.Matches() == ref.Matches()).all() and (half_.AcceptMasks() == ref.AcceptMasks()).all() \
+        and (half_.States() == ref.States()).all()
+print("ok pair_lines", flush=True)
 torch.cuda.synchronize()
 print("sanitize_run done, launches:", N.lib.pire_gpu_launch_count())
