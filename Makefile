@@ -9,8 +9,9 @@ NVCCFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -Wall 
 
 CSRC      := pire_b200/csrc
 LIB       := pire_b200/libpire_b200.so
-LIB_SRC   := $(CSRC)/pire_image.cpp $(CSRC)/dfa_tables.cpp $(CSRC)/scan_kernels.cu $(CSRC)/capi.cu $(CSRC)/capi_host.cu $(CSRC)/capi_dist.cu
-LIB_HDR   := $(CSRC)/capi_internal.hpp $(CSRC)/pire_image.hpp $(CSRC)/dfa_tables.hpp $(CSRC)/scan_kernels.cuh $(CSRC)/synth.h $(CSRC)/stage_copy.hpp include/pire_b200.h
+LIB_SRC   := $(CSRC)/pire_image.cpp $(CSRC)/dfa_tables.cpp $(CSRC)/scan_kernels.cu $(CSRC)/capi.cu $(CSRC)/capi_host.cu $(CSRC)/capi_dist.cu \
+            $(CSRC)/slow_image.cpp $(CSRC)/capi_slow.cu
+LIB_HDR   := $(CSRC)/capi_internal.hpp $(CSRC)/pire_image.hpp $(CSRC)/dfa_tables.hpp $(CSRC)/scan_kernels.cuh $(CSRC)/synth.h $(CSRC)/stage_copy.hpp $(CSRC)/slow_image.hpp include/pire_b200.h
 
 ORACLE    := oracle/libpire_oracle.so
 

@@ -698,6 +698,59 @@ int      pire_gpu_dead(const pire_gpu_scanner* sc, uint32_t state);             
 size_t   pire_gpu_accepted_regexps(const pire_gpu_scanner* sc, uint32_t state,
                                    uint32_t* ids, size_t cap);                           /* AcceptedRegexps multi.h:149-158 */
 
+/* ---- Pire::SlowScanner: patterns that cannot be determinised ---------------------
+ * Replaces, for every string i of a batch,
+ *     Pire::Runner(sc[, st_i]) [.Begin()] .Run(string i) [.End()]                          run.h:365-392
+ * on a Pire::SlowScanner (slow.h:43-50), the scanner Pire::Regexp falls back to when Fsm::Determine() fails
+ * (easy.h:205-215): x.{40}$, foo.{64}bar, approximate matching.  Its state is a SET of NFA states; here a set is W =
+ * ceil(Size() / 32) u32 words, bit s of word s / 32 = state s in the reference's numbering (SlowScanner::State's flags).
+ *   Create  `image` is the SlowScanner::Save() stream (header type 3; scanner_io.cpp:71-110).  Rejected with
+ *           PIRE_GPU_EIMAGE: what SlowScanner::Load / Mmap reject, and a start, jump or letter outside the automaton, jump
+ *           positions that step back or past the image, no states or no letters.  More than 4096 states is
+ *           PIRE_GPU_EUNSUPPORTED.  An image of SlowScanner::Null() (Empty(), slow.h:427-431) has one state and never
+ *           matches.  device == -1 builds a host-only handle (the host concept below; runs get PIRE_GPU_ENODEVICE).
+ *           pire_gpu_scanner_create refuses SlowScanner images, as before.
+ *   Batch   as pire_gpu_run_batch: CSR (d_offsets) or fixed length; with PIRE_GPU_RUN_LINES the offsets come from
+ *           pire_gpu_split_lines and string i ends one byte before offsets[i+1].
+ *   Start   d_start_sets NULL: Initialize() = {start}.  Otherwise n rows of W words; string i starts from row i
+ *           (Runner(sc, st_i)); bits at or past Size() in a row are ignored.  BEGIN steps BeginMark from each start.
+ *   Chain   d_sets may be d_start_sets: a batch of streams is carried on in place round after round, no synchronise.
+ *   Output  each may be NULL.  d_match_bits: ceil(n/32) words, bit (i%32) of word i/32 = Final() (slow.h:152-158), bits
+ *           past n are 0.  AcceptedRegexps() is {0} exactly when the bit is set (slow.h:165-167).  d_sets: n rows of W
+ *           words, the set after End() (after the bytes without END), bits past Size() 0.
+ *   flags   PIRE_GPU_RUN_BEGIN, PIRE_GPU_RUN_END, PIRE_GPU_RUN_LINES; anything else is PIRE_GPU_EINVAL, as are LINES with
+ *           start sets or without offsets, a NULL corpus with non-empty strings and n > 2^40.  n == 0 is a no-op.
+ * Scanners of at most 256 states walk one string per lane, larger ones one string per warp (DESIGN.md 4).  The walk of a
+ * string stops early when its set is empty (nothing can match any more); the results are what End() would give.
+ * Asynchronous on `stream`; re-entrant across streams on one handle. */
+typedef struct pire_gpu_slow_scanner pire_gpu_slow_scanner;
+
+typedef struct pire_gpu_slow_info {
+    uint32_t states;           /* SlowScanner::Size()             slow.h:83 */
+    uint32_t letters;          /* SlowScanner::GetLettersCount()  slow.h:81 */
+    uint32_t regexps;          /* RegexpsCount(): 0 when Empty(), else 1  slow.h:88 */
+    uint32_t set_words;        /* W = ceil(states / 32) */
+    uint32_t start;            /* Initialize()'s one state */
+    uint32_t empty;            /* Empty() */
+    uint64_t table_bytes;      /* device bytes of the successor rows */
+    uint64_t shared_bytes;     /* rows staged into shared memory per CTA (0: read through L1/L2) */
+    int32_t  device;           /* CUDA device, or -1 for a host-only handle */
+    uint32_t reserved;
+} pire_gpu_slow_info;
+
+int  pire_gpu_slow_scanner_create(const void* image, size_t size, int device, pire_gpu_slow_scanner** out);
+void pire_gpu_slow_scanner_destroy(pire_gpu_slow_scanner* sc);
+int  pire_gpu_slow_scanner_info(const pire_gpu_slow_scanner* sc, pire_gpu_slow_info* out);
+int  pire_gpu_slow_run_batch(const pire_gpu_slow_scanner* sc,
+                             const uint8_t* d_corpus, const uint64_t* d_offsets, uint64_t fixed_len, uint64_t n,
+                             uint32_t flags, const uint32_t* d_start_sets,
+                             uint32_t* d_match_bits, uint32_t* d_sets, void* stream);
+/* Host-side concept on the parsed tables, sets of W words (bits past Size() in an input are ignored). */
+int  pire_gpu_slow_initial(const pire_gpu_slow_scanner* sc, uint32_t* set);                  /* Initialize slow.h:91-97 */
+int  pire_gpu_slow_next(const pire_gpu_slow_scanner* sc, const uint32_t* set, uint32_t ch,
+                        uint32_t* out);                                                       /* Next slow.h:132-135; ch 0..259 */
+int  pire_gpu_slow_final(const pire_gpu_slow_scanner* sc, const uint32_t* set);             /* Final slow.h:152-158: 1 or 0 */
+
 /* ---- deterministic synthetic corpora (bench + tests) ---------------------------
  * Counter-based generator, identical bytes on host and device (SURVEY.md 8(d)).
  * kind 0: printable ASCII 0x20..0x7E; every `plant_every`-th string carries one

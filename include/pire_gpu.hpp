@@ -911,5 +911,137 @@ inline void MatchesHost(const Scanner& sc, const uint8_t* corpus, const uint64_t
         matched[i] = (bits[i / 32] >> (i % 32)) & 1u;
 }
 
+// Pire::SlowScanner (scanners/slow.h:43-50), the scanner Pire::Regexp falls back to when Fsm::Determine() fails.  Its
+// State is a set of NFA states: SetWords() u32 words, bit s % 32 of word s / 32 = state s in the reference's numbering
+// (SlowScanner::State's flags).  The host concept below steps such sets on the parsed tables, so the reference's own
+// Pire::Step / Pire::Run / Pire::Runner compile against it; the batch path runs on the device (SlowBatchRunner).
+class SlowScanner {
+public:
+    typedef std::vector<uint32_t> State;
+    typedef uint32_t Action;
+    typedef unsigned short Char;     // Pire::Char, pire/defs.h:59
+
+    SlowScanner() : Handle(nullptr) {}
+
+    // From a SlowScanner::Save() stream (scanner_io.cpp:71-110).  device = -1: host only.
+    SlowScanner(const void* image, size_t size, int device = 0) : Handle(nullptr)
+    {
+        Check(pire_gpu_slow_scanner_create(image, size, device, &Handle), "pire_gpu_slow_scanner_create");
+    }
+
+    // From a Pire::SlowScanner (or anything whose Save() writes that stream).
+    template <class PireSlowScanner>
+    explicit SlowScanner(const PireSlowScanner& sc, int device = 0) : Handle(nullptr)
+    {
+        std::ostringstream out;
+        sc.Save(&out);
+        const std::string image = out.str();
+        Check(pire_gpu_slow_scanner_create(image.data(), image.size(), device, &Handle), "pire_gpu_slow_scanner_create");
+    }
+
+    static SlowScanner Load(const void* image, size_t size, int device = 0) { return SlowScanner(image, size, device); }
+
+    SlowScanner(SlowScanner&& o) noexcept : Handle(o.Handle) { o.Handle = nullptr; }
+    SlowScanner& operator=(SlowScanner&& o) noexcept
+    {
+        if (this != &o) {
+            pire_gpu_slow_scanner_destroy(Handle);
+            Handle = o.Handle;
+            o.Handle = nullptr;
+        }
+        return *this;
+    }
+    SlowScanner(const SlowScanner&) = delete;
+    SlowScanner& operator=(const SlowScanner&) = delete;
+    ~SlowScanner() { pire_gpu_slow_scanner_destroy(Handle); }
+
+    size_t Size() const { return Info().states; }                        // slow.h:83
+    bool Empty() const { return Info().empty != 0; }                     // slow.h:85
+    size_t RegexpsCount() const { return Info().regexps; }               // slow.h:88
+    size_t LettersCount() const { return Info().letters; }               // slow.h:81
+    size_t SetWords() const { return Info().set_words; }
+
+    // ---- concept (host) ---------------------------------------------------------
+    void Initialize(State& st) const                                      // slow.h:91-97
+    {
+        st.assign(SetWords(), 0);
+        Check(pire_gpu_slow_initial(Handle, st.data()), "pire_gpu_slow_initial");
+    }
+    Action Next(State& st, Char c) const                                  // slow.h:132-140
+    {
+        State out(st.size());
+        Check(pire_gpu_slow_next(Handle, st.data(), c, out.data()), "pire_gpu_slow_next");
+        st.swap(out);
+        return 0;
+    }
+    void TakeAction(State&, Action) const {}
+    bool Final(const State& st) const                                     // slow.h:152-158
+    {
+        const int rc = pire_gpu_slow_final(Handle, st.data());
+        if (rc < 0)
+            Check(rc, "pire_gpu_slow_final");
+        return rc != 0;
+    }
+    bool Dead(const State&) const { return false; }                      // slow.h:160-163
+
+    pire_gpu_slow_info Info() const
+    {
+        pire_gpu_slow_info info;
+        Check(pire_gpu_slow_scanner_info(Handle, &info), "pire_gpu_slow_scanner_info");
+        return info;
+    }
+
+    pire_gpu_slow_scanner* Raw() const { return Handle; }
+
+private:
+    pire_gpu_slow_scanner* Handle;
+};
+
+// Runner(slow[, sets]) [.Begin()] .Run(batch) [.End()] for every string of a device batch (pire_gpu_slow_run_batch).
+// From(d_sets) starts string i from row i of n x SetWords() device words; the set output may be the same buffer, so a
+// batch of streams is carried on in place:
+//     Runner(slow, SlowBatchRunner::From(d_sets)).Run(piece_k).Launch(nullptr, d_sets);          // round k
+// Launch(d_match_bits, d_sets): Final() packed per string, and the set after End(); either may be null.
+class SlowBatchRunner {
+public:
+    struct StartSets {
+        explicit StartSets(const uint32_t* d_words) : Words(d_words) {}
+        const uint32_t* Words;
+    };
+    static StartSets From(const uint32_t* d_sets) { return StartSets(d_sets); }
+
+    explicit SlowBatchRunner(const SlowScanner& sc) : Sc(&sc), Start(nullptr), Flags(0), Ran(false) {}
+    SlowBatchRunner(const SlowScanner& sc, StartSets start) : SlowBatchRunner(sc)
+    {
+        if (!start.Words)
+            throw Error(PIRE_GPU_EINVAL, "SlowBatchRunner::From needs device words");
+        Start = start.Words;
+    }
+
+    SlowBatchRunner& Begin() { Flags |= PIRE_GPU_RUN_BEGIN; return *this; }
+    SlowBatchRunner& End() { Flags |= PIRE_GPU_RUN_END; return *this; }
+    SlowBatchRunner& Run(const Batch& b) { Input = b; Ran = true; return *this; }
+    SlowBatchRunner& Run(const LineFrame& f) { Input = f; Flags |= PIRE_GPU_RUN_LINES; Ran = true; return *this; }
+
+    void Launch(uint32_t* d_match_bits, uint32_t* d_sets, void* stream = nullptr) const
+    {
+        if (!Ran)
+            throw Error(PIRE_GPU_EINVAL, "SlowBatchRunner::Run() was not called");
+        Check(pire_gpu_slow_run_batch(Sc->Raw(), Input.Corpus, Input.Offsets, Input.FixedLen, Input.Count, Flags, Start,
+                                      d_match_bits, d_sets, stream),
+              "pire_gpu_slow_run_batch");
+    }
+
+private:
+    const SlowScanner* Sc;
+    const uint32_t* Start;
+    Batch Input;
+    unsigned Flags;
+    bool Ran;
+};
+
+inline SlowBatchRunner Runner(const SlowScanner& sc) { return SlowBatchRunner(sc); }
+inline SlowBatchRunner Runner(const SlowScanner& sc, SlowBatchRunner::StartSets start) { return SlowBatchRunner(sc, start); }
+
 } // namespace Gpu
 } // namespace Pire

@@ -43,6 +43,8 @@ SYMBOLS = [
     "pire_gpu_match_ends_lines", "pire_gpu_match_starts_lines",
     "pire_gpu_line_stream_create", "pire_gpu_line_stream_feed", "pire_gpu_line_stream_destroy",
     "pire_gpu_run_pair_lines",
+    "pire_gpu_slow_scanner_create", "pire_gpu_slow_scanner_destroy", "pire_gpu_slow_scanner_info", "pire_gpu_slow_run_batch",
+    "pire_gpu_slow_initial", "pire_gpu_slow_next", "pire_gpu_slow_final",
 ]
 
 
@@ -51,6 +53,12 @@ class Info(C.Structure):
                 ("empty", C.c_uint32), ("hot_rows", C.c_uint32), ("variant", C.c_uint32), ("tuned", C.c_uint32),
                 ("table_bytes", C.c_uint64), ("shared_bytes", C.c_uint64), ("device", C.c_int32),
                 ("reserved", C.c_uint32)]
+
+
+class SlowInfo(C.Structure):
+    _fields_ = [("states", C.c_uint32), ("letters", C.c_uint32), ("regexps", C.c_uint32), ("set_words", C.c_uint32),
+                ("start", C.c_uint32), ("empty", C.c_uint32), ("table_bytes", C.c_uint64), ("shared_bytes", C.c_uint64),
+                ("device", C.c_int32), ("reserved", C.c_uint32)]
 
 
 class LineFrame(C.Structure):
@@ -143,6 +151,14 @@ def _load():
     lib.pire_gpu_comm_wait.argtypes = [vp, vp]
     lib.pire_gpu_comm_gather_bits.argtypes = [vp, C.c_uint64, vp, C.c_uint32, vp]
     lib.pire_gpu_run_sharded.argtypes = [vp, vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp]
+    lib.pire_gpu_slow_scanner_create.argtypes = [vp, C.c_size_t, C.c_int, C.POINTER(vp)]
+    lib.pire_gpu_slow_scanner_destroy.argtypes = [vp]
+    lib.pire_gpu_slow_scanner_destroy.restype = None
+    lib.pire_gpu_slow_scanner_info.argtypes = [vp, C.POINTER(SlowInfo)]
+    lib.pire_gpu_slow_run_batch.argtypes = [vp, vp, vp, C.c_uint64, C.c_uint64, C.c_uint32, vp, vp, vp, vp]
+    lib.pire_gpu_slow_initial.argtypes = [vp, vp]
+    lib.pire_gpu_slow_next.argtypes = [vp, vp, C.c_uint32, vp]
+    lib.pire_gpu_slow_final.argtypes = [vp, vp]
     return lib
 
 

@@ -5685,6 +5685,363 @@ cudaError_t LaunchAcceptGather(const uint32_t* d_table, uint32_t states, uint32_
     return cudaGetLastError();
 }
 
+// ---------------------------------------------------------------- SlowScanner: a set of NFA states per string
+//
+// Pire::SlowScanner (slow.h:43-50) steps a SET of NFA states on each byte: next = the union of the successor rows of
+// the states in the set, on the byte's letter (NextTranslated, slow.h:103-130).  Here a set is a bit set of W = ceil(S/32)
+// words in the reference's numbering, and succ[(l * S + s) * stride ..] is the successor set of state s on letter l.
+// Dead() is always false in the reference, but an empty set stays empty: a warp whose sets are all empty stops reading.
+//   * Lane path (S <= 256): one string per lane, its set in kW registers (kW = 1, 2, 4, 8; stride kW).  A step walks
+//     the set bits and ORs in each row with one vector load.  Input: aligned 16-byte chunks through LoadChunk16 (read
+//     only, clipped at the corpus edges), handed out byte by byte as in the generic kernel's edges.
+//   * Warp path (256 < S <= 4096): one string per warp, lane l owns words l, l + 32, .. (kJ per lane; stride W).  The
+//     warp finds the non-empty words with a ballot, broadcasts each, and reads every active state's row as one coalesced
+//     load.  Each lane loads one 16-byte chunk of a 512-byte window of the string; the chunks are broadcast in turn.
+//     Warps take strings grid-stride and OR their match bits into words the launch zeroed.
+// Both paths read the rows from shared memory when the table fits the CTA budget (SlowArgs::shared_rows), else through
+// L1/L2; the pointer is generic.
+
+namespace {
+
+constexpr int kSlowBlock = 256;
+constexpr int kSlowLaneBlocksPerSM = 3;
+constexpr int kSlowWarpBlocksPerSM = 4;
+constexpr size_t kSlowClsBytes = 528;     // 260 u16 letters, padded to 16
+
+// The CTA's copy of the letters (and, with shared_rows, the rows); returns the rows the walk reads.
+__device__ __forceinline__ const uint32_t* SlowStage(const SlowArgs& a, const uint16_t*& cls)
+{
+    uint32_t* rows = reinterpret_cast<uint32_t*>(pire_b200_smem);
+    uint16_t* c = reinterpret_cast<uint16_t*>(pire_b200_smem + a.shared_rows);
+    for (uint32_t k = threadIdx.x; k < 260; k += blockDim.x)
+        c[k] = a.cls[k];
+    for (uint32_t k = threadIdx.x; k < a.shared_rows / 4; k += blockDim.x)
+        rows[k] = __ldg(a.succ + k);
+    __syncthreads();
+    cls = c;
+    return a.shared_rows ? rows : a.succ;
+}
+
+__device__ __forceinline__ void SlowBounds(const SlowArgs& a, uint64_t i, uint64_t& b, uint64_t& e)
+{
+    if (a.offsets) {
+        b = a.offsets[i];
+        e = a.offsets[i + 1] - a.trim;
+        e = e < b ? b : e;
+    } else {
+        b = i * a.fixed_len;
+        e = b + a.fixed_len;
+    }
+}
+
+// bits of word w at or past S cleared
+__device__ __forceinline__ uint32_t SlowKeep(uint32_t states, uint32_t w)
+{
+    const uint32_t lo = w * 32;
+    return lo >= states ? 0u : states - lo >= 32 ? ~0u : (1u << (states - lo)) - 1;
+}
+
+template <int kW>
+__device__ __forceinline__ void SlowLaneStep(const uint32_t* rows, uint32_t states, uint32_t letter, uint32_t (&cur)[kW])
+{
+    const uint32_t* base = rows + (size_t) letter * states * kW;
+    uint32_t nx[kW];
+#pragma unroll
+    for (int w = 0; w < kW; ++w)
+        nx[w] = 0;
+#pragma unroll
+    for (int w = 0; w < kW; ++w) {
+        uint32_t bits = cur[w];
+        while (bits) {
+            const uint32_t s = w * 32 + __ffs(bits) - 1;
+            bits &= bits - 1;
+            const uint32_t* r = base + s * kW;
+            if (kW == 1) {
+                nx[0] |= r[0];
+            } else if (kW == 2) {
+                const uint2 v = *reinterpret_cast<const uint2*>(r);
+                nx[0] |= v.x;
+                nx[1 % kW] |= v.y;
+            } else {
+#pragma unroll
+                for (int q = 0; q < kW / 4; ++q) {
+                    const uint4 v = *reinterpret_cast<const uint4*>(r + 4 * q);
+                    nx[(4 * q) % kW] |= v.x;
+                    nx[(4 * q + 1) % kW] |= v.y;
+                    nx[(4 * q + 2) % kW] |= v.z;
+                    nx[(4 * q + 3) % kW] |= v.w;
+                }
+            }
+        }
+    }
+#pragma unroll
+    for (int w = 0; w < kW; ++w)
+        cur[w] = nx[w];
+}
+
+template <int kW>
+__device__ __forceinline__ bool SlowAny(const uint32_t (&cur)[kW])
+{
+    uint32_t any = 0;
+#pragma unroll
+    for (int w = 0; w < kW; ++w)
+        any |= cur[w];
+    return any != 0;
+}
+
+template <int kW>
+__global__ void __launch_bounds__(kSlowBlock, kSlowLaneBlocksPerSM) SlowLaneKernel(const __grid_constant__ SlowArgs a)
+{
+    const uint16_t* cls;
+    const uint32_t* rows = SlowStage(a, cls);
+    uint32_t fm[kW];
+#pragma unroll
+    for (int w = 0; w < kW; ++w)
+        fm[w] = w < (int) a.words ? a.final_mask[w] : 0;
+
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t units = (a.n + 31) / 32;
+    const uint64_t warps = (uint64_t) gridDim.x * (kSlowBlock / 32);
+    const uintptr_t buf_lo = reinterpret_cast<uintptr_t>(a.corpus);
+    const uintptr_t buf_hi = buf_lo + (a.offsets ? a.offsets[a.n] - a.trim : a.n * a.fixed_len);
+
+    for (uint64_t unit = (uint64_t) blockIdx.x * (kSlowBlock / 32) + (threadIdx.x >> 5); unit < units; unit += warps) {
+        const uint64_t i = unit * 32 + lane;
+        const bool valid = i < a.n;
+        uint64_t b = 0, e = 0;
+        if (valid)
+            SlowBounds(a, i, b, e);
+        uint32_t cur[kW];
+#pragma unroll
+        for (int w = 0; w < kW; ++w) {
+            if (a.start_sets)
+                cur[w] = valid && w < (int) a.words ? a.start_sets[i * a.words + w] & SlowKeep(a.states, w) : 0;
+            else
+                cur[w] = valid && (uint32_t) w == a.start / 32 ? 1u << (a.start % 32) : 0;
+        }
+        if (a.with_begin)
+            SlowLaneStep<kW>(rows, a.states, cls[258], cur);
+
+        const uint8_t* p = a.corpus + b;
+        const uint8_t* end = a.corpus + e;
+        const uint8_t* chunk = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(p) & ~uintptr_t(15));
+        while (__any_sync(0xffffffffu, chunk < end && SlowAny<kW>(cur))) {
+            if (chunk < end && SlowAny<kW>(cur)) {
+                const uint32_t skip = p > chunk ? (uint32_t) (p - chunk) : 0;
+                const uint32_t stop = end < chunk + 16 ? (uint32_t) (end - chunk) : 16;
+                EdgeBytes eb(LoadChunk16(chunk, buf_lo, buf_hi), skip);
+                for (uint32_t k = skip; k < stop; ++k)
+                    SlowLaneStep<kW>(rows, a.states, cls[eb.Next()], cur);
+            }
+            chunk += 16;
+        }
+        if (a.with_end)
+            SlowLaneStep<kW>(rows, a.states, cls[259], cur);
+
+        uint32_t hit = 0;
+#pragma unroll
+        for (int w = 0; w < kW; ++w)
+            hit |= cur[w] & fm[w];
+        const uint32_t bits = __ballot_sync(0xffffffffu, valid && hit != 0);
+        if (a.match_bits && lane == 0)
+            a.match_bits[unit] = bits;
+        if (a.sets && valid) {
+#pragma unroll
+            for (int w = 0; w < kW; ++w)
+                if (w < (int) a.words)
+                    a.sets[i * a.words + w] = cur[w];
+        }
+    }
+}
+
+template <int kJ>
+__device__ __forceinline__ void SlowWarpStep(const uint32_t* rows, uint32_t states, uint32_t words, uint32_t letter, uint32_t lane,
+                                             uint32_t (&cur)[kJ])
+{
+    const uint32_t* base = rows + (size_t) letter * states * words + lane;
+    uint32_t nx[kJ];
+#pragma unroll
+    for (int j = 0; j < kJ; ++j)
+        nx[j] = 0;
+#pragma unroll
+    for (int j = 0; j < kJ; ++j) {
+        uint32_t act = __ballot_sync(0xffffffffu, cur[j] != 0);
+        while (act) {
+            const uint32_t src = __ffs(act) - 1;
+            act &= act - 1;
+            uint32_t bits = __shfl_sync(0xffffffffu, cur[j], src);
+            const uint32_t first = (j * 32 + src) * 32;
+            while (bits) {
+                const uint32_t s = first + __ffs(bits) - 1;
+                bits &= bits - 1;
+                const uint32_t* r = base + (size_t) s * words;
+#pragma unroll
+                for (int q = 0; q < kJ; ++q)
+                    if (lane + 32 * q < words)
+                        nx[q] |= r[32 * q];
+            }
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < kJ; ++j)
+        cur[j] = nx[j];
+}
+
+template <int kJ>
+__global__ void __launch_bounds__(kSlowBlock, kSlowWarpBlocksPerSM) SlowWarpKernel(const __grid_constant__ SlowArgs a)
+{
+    const uint16_t* cls;
+    const uint32_t* rows = SlowStage(a, cls);
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t fm[kJ];
+#pragma unroll
+    for (int j = 0; j < kJ; ++j)
+        fm[j] = lane + 32 * j < a.words ? a.final_mask[lane + 32 * j] : 0;
+
+    const uint64_t warps = (uint64_t) gridDim.x * (kSlowBlock / 32);
+    const uintptr_t buf_lo = reinterpret_cast<uintptr_t>(a.corpus);
+    const uintptr_t buf_hi = buf_lo + (a.offsets ? a.offsets[a.n] - a.trim : a.n * a.fixed_len);
+
+    // one string per warp, handed out grid-stride; the match bit goes in with an atomic OR (the launch zeroed the words)
+    for (uint64_t i = (uint64_t) blockIdx.x * (kSlowBlock / 32) + (threadIdx.x >> 5); i < a.n; i += warps) {
+        uint64_t b, e;
+        SlowBounds(a, i, b, e);
+        uint32_t cur[kJ];
+#pragma unroll
+        for (int j = 0; j < kJ; ++j) {
+            const uint32_t w = lane + 32 * j;
+            if (a.start_sets)
+                cur[j] = w < a.words ? a.start_sets[i * a.words + w] & SlowKeep(a.states, w) : 0;
+            else
+                cur[j] = w == a.start / 32 ? 1u << (a.start % 32) : 0;
+        }
+        if (a.with_begin)
+            SlowWarpStep<kJ>(rows, a.states, a.words, cls[258], lane, cur);
+
+        const uint8_t* p = a.corpus + b;
+        const uint8_t* end = a.corpus + e;
+        const uint8_t* window = reinterpret_cast<const uint8_t*>(reinterpret_cast<uintptr_t>(p) & ~uintptr_t(15));
+        bool alive = true;
+        for (; window < end && alive; window += 512) {
+            const uint8_t* mine = window + 16 * lane;
+            const uint4 v = mine < end ? LoadChunk16(mine, buf_lo, buf_hi) : make_uint4(0, 0, 0, 0);
+            for (uint32_t c = 0; c < 32 && alive; ++c) {
+                const uint8_t* chunk = window + 16 * c;
+                if (chunk >= end)
+                    break;
+                const uint4 w = make_uint4(__shfl_sync(0xffffffffu, v.x, c), __shfl_sync(0xffffffffu, v.y, c),
+                                           __shfl_sync(0xffffffffu, v.z, c), __shfl_sync(0xffffffffu, v.w, c));
+                const uint32_t skip = p > chunk ? (uint32_t) (p - chunk) : 0;
+                const uint32_t stop = end < chunk + 16 ? (uint32_t) (end - chunk) : 16;
+                EdgeBytes eb(w, skip);
+                for (uint32_t t = skip; t < stop; ++t)
+                    SlowWarpStep<kJ>(rows, a.states, a.words, cls[eb.Next()], lane, cur);
+                uint32_t any = 0;
+#pragma unroll
+                for (int j = 0; j < kJ; ++j)
+                    any |= cur[j];
+                alive = __any_sync(0xffffffffu, any != 0);
+            }
+        }
+        if (a.with_end)
+            SlowWarpStep<kJ>(rows, a.states, a.words, cls[259], lane, cur);
+        uint32_t hit = 0;
+#pragma unroll
+        for (int j = 0; j < kJ; ++j)
+            hit |= cur[j] & fm[j];
+        if (__any_sync(0xffffffffu, hit != 0) && a.match_bits && lane == 0)
+            atomicOr(a.match_bits + i / 32, 1u << (i % 32));
+        if (a.sets) {
+#pragma unroll
+            for (int j = 0; j < kJ; ++j)
+                if (lane + 32 * j < a.words)
+                    a.sets[i * a.words + lane + 32 * j] = cur[j];
+        }
+    }
+}
+
+struct SlowKernel {
+    const void* fn;
+    int per_sm;
+};
+
+SlowKernel SlowKernelFor(uint32_t states, uint32_t words)
+{
+    if (states <= kSlowLaneMaxStates) {
+        if (words <= 1)
+            return {reinterpret_cast<const void*>(&SlowLaneKernel<1>), kSlowLaneBlocksPerSM};
+        if (words <= 2)
+            return {reinterpret_cast<const void*>(&SlowLaneKernel<2>), kSlowLaneBlocksPerSM};
+        if (words <= 4)
+            return {reinterpret_cast<const void*>(&SlowLaneKernel<4>), kSlowLaneBlocksPerSM};
+        return {reinterpret_cast<const void*>(&SlowLaneKernel<8>), kSlowLaneBlocksPerSM};
+    }
+    if (words <= 32)
+        return {reinterpret_cast<const void*>(&SlowWarpKernel<1>), kSlowWarpBlocksPerSM};
+    if (words <= 64)
+        return {reinterpret_cast<const void*>(&SlowWarpKernel<2>), kSlowWarpBlocksPerSM};
+    return {reinterpret_cast<const void*>(&SlowWarpKernel<4>), kSlowWarpBlocksPerSM};
+}
+
+} // namespace
+
+uint32_t SlowRowStride(uint32_t states, uint32_t words)
+{
+    if (states > kSlowLaneMaxStates)
+        return words;
+    return words <= 1 ? 1 : words <= 2 ? 2 : words <= 4 ? 4 : 8;
+}
+
+size_t SlowSharedBytes(uint64_t table_bytes, int device)
+{
+    int optin = 0, per_sm = 0;
+    if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess
+        || cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, device) != cudaSuccess)
+        return 0;
+    // the rows go to shared memory when two CTAs of the kernel still fit on an SM
+    const uint64_t budget = (uint64_t) per_sm / 2 - 1024 - kSlowClsBytes;
+    return table_bytes <= budget && table_bytes + kSlowClsBytes <= (uint64_t) optin ? (size_t) table_bytes : 0;
+}
+
+cudaError_t LaunchSlow(const SlowArgs& a, int device, cudaStream_t stream)
+{
+    if (a.n == 0)
+        return cudaSuccess;
+    const SlowKernel k = SlowKernelFor(a.states, a.words);
+    const size_t shared = a.shared_rows + kSlowClsBytes;
+    // the device's opt-in limit, the same value from every call: concurrent launches of other handles on other streams
+    // never lower the limit under one another
+    int optin = 0, sms = 0, per_sm = 0;
+    cudaError_t err = cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device);
+    if (err == cudaSuccess)
+        err = cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+    if (err == cudaSuccess)
+        err = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    if (err == cudaSuccess)
+        err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k.fn, kSlowBlock, shared);
+    if (err != cudaSuccess)
+        return err;
+    if (per_sm < 1)
+        return cudaErrorLaunchOutOfResources;
+    // the lane path has a warp per 32 strings and writes whole match words; the warp path has a warp per string and ORs
+    // its bit into words zeroed here
+    const bool lane_path = a.states <= kSlowLaneMaxStates;
+    const uint64_t warps = lane_path ? (a.n + 31) / 32 : a.n;
+    const uint64_t want = (warps + kSlowBlock / 32 - 1) / (kSlowBlock / 32);
+    const uint64_t cap = (uint64_t) sms * (uint64_t) per_sm;
+    if (!lane_path && a.match_bits) {
+        err = cudaMemsetAsync(a.match_bits, 0, (a.n + 31) / 32 * sizeof(uint32_t), stream);
+        if (err != cudaSuccess)
+            return err;
+    }
+    SlowArgs copy = a;
+    void* args[] = {&copy};
+    err = cudaLaunchKernel(k.fn, dim3((unsigned) (want < cap ? want : cap)), dim3(kSlowBlock), args, shared, stream);
+    if (err == cudaSuccess)
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+    return err;
+}
+
 uint64_t KernelLaunchCount() { return g_launches.load(std::memory_order_relaxed); }
 
 } // namespace pire_b200

@@ -201,6 +201,37 @@ cudaError_t LaunchSynthMixedFill(uint64_t seed, uint32_t plant_every, uint64_t f
 cudaError_t LaunchAcceptGather(const uint32_t* d_table, uint32_t states, uint32_t words, const uint32_t* d_state_idx, uint64_t n,
                                uint32_t* d_out, cudaStream_t stream);
 
+// Pire::SlowScanner over a batch (SlowLaneKernel / SlowWarpKernel, pire_gpu_slow_run_batch): every string's set of NFA
+// states, from {start} or its own start set, marks as with_begin / with_end, Final() packed into match_bits and the set
+// after End() into sets (each may be null).  Device pointers.
+struct SlowArgs {
+    const uint8_t* corpus;
+    const uint64_t* offsets;     // CSR (n+1) or nullptr
+    uint32_t trim;               // 1: the offsets are lines from SplitLines
+    uint64_t fixed_len;
+    uint64_t n;
+    const uint16_t* cls;         // [260]: letter of each byte and mark
+    const uint32_t* succ;        // [letters][states][SlowRowStride] successor sets
+    const uint32_t* final_mask;  // [words]
+    uint32_t states;
+    uint32_t words;              // ceil(states / 32)
+    uint32_t start;              // Initialize()'s state
+    uint32_t with_begin;
+    uint32_t with_end;
+    uint32_t shared_rows;        // bytes of succ staged into shared memory (0: read through L1/L2)
+    const uint32_t* start_sets;  // n rows of `words`, or null: {start}
+    uint32_t* match_bits;        // ceil(n/32) words, or null
+    uint32_t* sets;              // n rows of `words`, or null; may be start_sets
+};
+// states up to this walk one string per lane; above it (to kSlowMaxStates) one string per warp
+constexpr uint32_t kSlowLaneMaxStates = 256;
+constexpr uint32_t kSlowMaxStates = 4096;
+// u32 words between two successor rows of the kernel a scanner of `states` runs
+uint32_t SlowRowStride(uint32_t states, uint32_t words);
+// bytes of a table of `table_bytes` that the launch stages into shared memory: all of it or none
+size_t SlowSharedBytes(uint64_t table_bytes, int device);
+cudaError_t LaunchSlow(const SlowArgs& a, int device, cudaStream_t stream);
+
 uint64_t KernelLaunchCount();
 
 } // namespace pire_b200

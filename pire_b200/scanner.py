@@ -7,6 +7,7 @@ Reference interface mirrored (same names and argument meaning):
                               StateIndex / Load          pire/scanners/multi.h:134-194,:244-311
     Pire::Runner(sc)          .Begin().Run(...).End()    pire/run.h:365-392
     Pire::Matches(sc, ...)    no Begin/End marks         pire/run.h:396-400
+    Pire::SlowScanner         the same Runner surface, its state a set of NFA states   pire/scanners/slow.h
 
 The one difference is the unit of work: Run() takes a *batch* of strings
 resident in HBM (``Batch``) instead of one ``const char*`` range, and the
@@ -1267,11 +1268,143 @@ def MatchStarts(rsc, ends, window, base=0, begin=True, end=True, max_back=0):
     return MatchStartsResult(ends, starts, open_)
 
 
+class SlowScanner:
+    """A compiled Pire::SlowScanner (slow.h:43-50) on one GPU: the scanner Pire::Regexp falls back to when a pattern cannot
+    be determinised.  Its state is a set of NFA states, here a numpy uint32 array of ``set_words`` words (bit s of word
+    s // 32 = state s, the reference's numbering).  ``device`` -1 makes a host-only handle: the host concept works, runs
+    raise."""
+
+    def __init__(self, image, device=0):
+        image = bytes(image)
+        h = C.c_void_p()
+        buf = (C.c_char * len(image)).from_buffer_copy(image)
+        N.check(N.lib.pire_gpu_slow_scanner_create(buf, len(image), int(device), C.byref(h)), "pire_gpu_slow_scanner_create")
+        self._h = h
+        self.device = int(device)
+        self.set_words = self.info().set_words
+
+    @classmethod
+    def Load(cls, image, device=0):
+        return cls(image, device)
+
+    def __del__(self):
+        h = getattr(self, "_h", None)
+        lib = getattr(N, "lib", None)
+        if h and lib is not None:
+            lib.pire_gpu_slow_scanner_destroy(h)
+            self._h = None
+
+    def info(self):
+        out = N.SlowInfo()
+        N.check(N.lib.pire_gpu_slow_scanner_info(self._h, C.byref(out)), "pire_gpu_slow_scanner_info")
+        return out
+
+    def Size(self):
+        return self.info().states
+
+    def Empty(self):
+        return bool(self.info().empty)
+
+    def RegexpsCount(self):
+        return self.info().regexps
+
+    def LettersCount(self):
+        return self.info().letters
+
+    # --- host-side concept on sets ---------------------------------------------
+    def Initialize(self):
+        out = np.zeros(self.set_words, np.uint32)
+        N.check(N.lib.pire_gpu_slow_initial(self._h, out.ctypes.data), "pire_gpu_slow_initial")
+        return out
+
+    def Next(self, state, ch):
+        cur = np.ascontiguousarray(state, dtype=np.uint32)
+        if cur.size != self.set_words:
+            raise ValueError("a set has %d words" % self.set_words)
+        out = np.zeros(self.set_words, np.uint32)
+        N.check(N.lib.pire_gpu_slow_next(self._h, cur.ctypes.data, int(ch), out.ctypes.data), "pire_gpu_slow_next")
+        return out
+
+    def Final(self, state):
+        cur = np.ascontiguousarray(state, dtype=np.uint32)
+        if cur.size != self.set_words:
+            raise ValueError("a set has %d words" % self.set_words)
+        rc = N.lib.pire_gpu_slow_final(self._h, cur.ctypes.data)
+        if rc < 0:
+            N.check(rc, "pire_gpu_slow_final")
+        return bool(rc)
+
+    def AcceptedRegexps(self, state):
+        """{0} when Final(), else {} (slow.h:165-167)."""
+        return [0] if self.Final(state) else []
+
+    def run_batch(self, batch, flags, match_bits=None, sets=None, start_sets=None, stream=None):
+        """Thin wrapper of pire_gpu_slow_run_batch, asynchronous on the current stream.  ``start_sets`` (an int32 CUDA
+        tensor of n * set_words words) starts string i from row i; it may be ``sets`` itself, so that rounds of a batch of
+        streams chain in place.  A line batch (``trim`` 1) runs with PIRE_GPU_RUN_LINES."""
+        torch = _torch()
+        if stream is None:
+            stream = torch.cuda.current_stream(batch.device).cuda_stream
+        ptr = lambda t: None if t is None else t.data_ptr()
+        if getattr(batch, "order", None) is not None:
+            raise ValueError("a SlowScanner batch is not length-ordered")
+        if start_sets is not None:
+            if start_sets.dtype != torch.int32 or not start_sets.is_cuda or not start_sets.is_contiguous() \
+                    or start_sets.numel() < batch.n * self.set_words:
+                raise ValueError("start_sets must be a contiguous int32 CUDA tensor of n * set_words words")
+        if getattr(batch, "trim", 0):
+            flags |= N.RUN_LINES
+        N.check(N.lib.pire_gpu_slow_run_batch(self._h, batch.corpus.data_ptr(), ptr(batch.offsets), batch.fixed_len, batch.n,
+                                              flags, ptr(start_sets), ptr(match_bits), ptr(sets), stream),
+                "pire_gpu_slow_run_batch")
+
+
+class SlowRunHelper(RunHelper):
+    """Pire::RunHelper over a batch for a SlowScanner: ``Runner(slow)`` or ``Runner(slow, sets)`` with ``sets`` an int32
+    CUDA tensor of n * set_words words.  ``Matches()`` / ``MatchBits()`` as for a Scanner; ``Sets()`` is the set each
+    string ended in, an (n, set_words) uint32 array, and ``SetTensor()`` the device tensor to chain into the next round."""
+
+    def _launch(self):
+        if self._bits is not None:
+            return
+        if self._batch is None:
+            raise ValueError("Run() was not called")
+        torch = _torch()
+        b = self._batch
+        self._bits = torch.empty((b.n + 31) // 32, dtype=torch.int32, device=b.device)
+        self._states = torch.empty(b.n * self.Sc.set_words, dtype=torch.int32, device=b.device)
+        flags = (N.RUN_BEGIN if self._begin else 0) | (N.RUN_END if self._end else 0)
+        self.Sc.run_batch(b, flags, self._bits, self._states, start_sets=self._start)
+
+    def SetTensor(self):
+        self._launch()
+        return self._states
+
+    def Sets(self):
+        self._launch()
+        return self._states.cpu().numpy().view(np.uint32).reshape(self._batch.n, self.Sc.set_words)
+
+    def AcceptMasks(self):
+        """AcceptedRegexps() is {0} exactly when the match bit is set (slow.h:165-167)."""
+        return self.Matches().astype(np.uint32)
+
+    def States(self):
+        return self.Sets()
+
+    def StateTensor(self):
+        return self.SetTensor()
+
+    def AcceptedRegexps(self, i):
+        return [0] if self.Matches()[i] else []
+
+
 def Runner(sc, states=None):
     """Pire::Runner(sc) (run.h:388-389); with ``states`` Pire::Runner(sc, st) (run.h:391-392) for every string.  For a
     ScannerPair, ``states`` is a pair (states1, states2), either None."""
     if isinstance(sc, ScannerPair):
         return PairRunHelper(sc, states)
+    if isinstance(sc, SlowScanner):
+        return SlowRunHelper(sc, states)
     return RunHelper(sc, states)
 
 

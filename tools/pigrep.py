@@ -4,8 +4,10 @@
 
     python tools/pigrep.py --scanner patterns.pire file [file ...]     # precompiled Scanner::Save() image
     python tools/pigrep.py --scanner a.pire --scanner b.pire file ...  # a pattern set glued into two scanners
+    python tools/pigrep.py --scanner slow.pire file [file ...]          # a SlowScanner::Save() image (header type 3)
     python tools/pigrep.py [-i] [-u] -e PATTERN file [file ...]        # compile with the reference front end
-                                                                       # (needs oracle/_ref; developer convenience)
+                                                                       # (needs oracle/_ref and the reference tree;
+                                                                       # developer convenience)
     python tools/pigrep.py --half-final hf.pire --reverse rev.pire -o file [file ...]
     zcat x.gz | python tools/pigrep.py --scanner patterns.pire            # no file, or "-": standard input
 
@@ -30,6 +32,13 @@ ascending, then end descending, a span is taken when it starts at or after the e
 is close to what grep -o prints, but it is this selection over Pire's spans, not GNU grep's matcher, and the two can
 differ.  With -o, -c counts the lines that have at least one span, and --scanner is not used.  With -e all three
 scanners are compiled from the pattern.
+
+Patterns that cannot be determinised (x.{40}$, foo.{64}bar): --scanner reads the image's header type, and a
+Pire::SlowScanner image (type 3) runs pire_gpu_slow_run_batch over each frame's lines; -c, -n and -b keep their meaning.
+-e compiles the way Pire::Regexp does (easy.h:211-214): when Fsm::Determine() fails, the pattern becomes a SlowScanner
+built from the same Fsm (this needs the reference tree, $PIRE_REF, to build tests/golden/slow_ref.cpp; without it -e
+compiles a Scanner as before).  Match spans (-o) and pairs of scanners are DFA-only: with a SlowScanner, -o or a second
+--scanner exits with a message.
 """
 import argparse
 import os
@@ -37,6 +46,14 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+
+
+SLOW_SCANNER = 3          # ScannerIOTypes::SlowScanner, pire/scanners/common.h:38
+
+
+def image_type(image):
+    """The scanner type in an image's stream header (common.h:44-63), or 0 for a buffer too short to hold one."""
+    return int.from_bytes(image[16:20], "little") if len(image) >= 24 else 0
 
 
 def select_spans(spans):
@@ -83,16 +100,34 @@ def main():
     import pire_b200 as P
     images, hf_image, rev_image = [], None, None
     if args.pattern:
-        sys.path.insert(0, os.path.join(ROOT, "tests"))
-        from refpire import Ref           # the reference's own Lexer/Fsm/Compile, unchanged host code
-        ref, opts = Ref(), ("i" if args.i else "") + ("u" if args.u else "")
-        images = [ref.compile(args.pattern.encode(), opts).save()]
-        hf_image = ref.compile_half_final(args.pattern.encode(), opts).save()
-        rev_image = ref.compile(args.pattern.encode(), opts + "nr").save()
+        sys.path[:0] = [os.path.join(ROOT, "tests"), os.path.join(ROOT, "tests", "golden")]
+        import tempfile
+        from make_slow_images import REF, build_helper, compile_slow
+        opts = ("i" if args.i else "") + ("u" if args.u else "")
+        slow_image, determinable = None, True
+        if os.path.isdir(os.path.join(REF, "pire")):
+            # Pire::SlowScanner's C face is built against the reference tree; without the tree the pattern is compiled
+            # as a Scanner, as before
+            with tempfile.TemporaryDirectory() as tmp:
+                slow_image, determinable = compile_slow(build_helper(tmp), args.pattern.encode(), opts, max_size=0)
+        if not determinable:
+            images = [slow_image]
+        else:
+            from refpire import Ref           # the reference's own Lexer/Fsm/Compile, unchanged host code
+            ref = Ref()
+            images = [ref.compile(args.pattern.encode(), opts).save()]
+            hf_image = ref.compile_half_final(args.pattern.encode(), opts).save()
+            rev_image = ref.compile(args.pattern.encode(), opts + "nr").save()
     else:
         images = [open(name, "rb").read() for name in args.scanner]
         hf_image = open(args.half_final, "rb").read() if args.half_final else None
         rev_image = open(args.reverse, "rb").read() if args.reverse else None
+    slow = [image_type(image) == SLOW_SCANNER for image in images]
+    if any(slow) and args.o:
+        ap.error("-o prints match spans, which need DFA images: a SlowScanner (a pattern that cannot be determinised) "
+                 "gives matching lines only")
+    if any(slow) and len(images) > 1:
+        ap.error("a SlowScanner image runs alone: two scanners at once are DFA-only")
     if args.o and not (hf_image and rev_image):
         ap.error("-o needs --half-final FILE and --reverse FILE, or -e PATTERN")
     if not args.o and not images:
@@ -100,7 +135,7 @@ def main():
     if len(images) > 2:
         ap.error("--scanner may be given at most twice")
     block = max(1, int(args.block_mb * (1 << 20)))
-    scanners = [P.Scanner(image, 0) for image in images] if not args.o else []
+    scanners = [P.SlowScanner(image, 0) if k else P.Scanner(image, 0) for image, k in zip(images, slow)] if not args.o else []
     sc = scanners[0] if len(scanners) == 1 else P.ScannerPair(*scanners) if scanners else None
     hf = P.Scanner(hf_image, 0) if args.o else None
     rev = P.Scanner(rev_image, 0) if args.o else None
@@ -150,7 +185,8 @@ class HeldText:
 
 
 def grep_stream(P, args, sc, hf, rev, f, block, prefix, out):
-    """Greps one input; prints the matches and returns the -c count.  `sc` is a Scanner or a ScannerPair."""
+    """Greps one input; prints the matches and returns the -c count.  `sc` is a Scanner, a SlowScanner or a
+    ScannerPair."""
     import numpy as np
     ls = P.LineStream(0)
     held = HeldText()

@@ -327,5 +327,19 @@ for half_, one in ((both.First(), sc), (both.Second(), other)):
     assert (half_.Matches() == ref.Matches()).all() and (half_.AcceptMasks() == ref.AcceptMasks()).all() \
         and (half_.States() == ref.States()).all()
 print("ok pair_lines", flush=True)
+# a SlowScanner on both paths (pire_gpu_slow_run_batch): the reference's recorded answers, a CSR batch and lines of a text
+from slow_fixtures import SLOW
+for name in ("heavy/a30", "heavy/error200"):
+    e = next(x for x in SLOW if x.name == name)
+    ssc = P.SlowScanner(e.image, 0)
+    r = P.Runner(ssc).Begin().Run(P.Batch.from_strings(e.strings)).End()
+    final, sets = e.runs[(True, True, False)]
+    assert (r.Matches() == final).all() and (r.Sets() == sets).all(), name
+    text = b"\n".join(e.strings) + b"\n"          # the strings hold newlines of their own: compare line by line
+    lines = P.Batch.from_text(torch.tensor(list(text), dtype=torch.uint8, device=dev))
+    want = P.Runner(ssc).Begin().Run(P.Batch.from_strings(text.split(b"\n")[:-1])).End()
+    got = P.Runner(ssc).Begin().Run(lines).End()
+    assert (got.Matches() == want.Matches()).all() and (got.Sets() == want.Sets()).all(), name + " lines"
+print("ok slow_run_batch", flush=True)
 torch.cuda.synchronize()
 print("sanitize_run done, launches:", N.lib.pire_gpu_launch_count())
